@@ -1,4 +1,4 @@
-"""adflow_b200 -- B200-native (sm_100a CUDA) drop-in for ADflow's per-block
+"""adflow_b200 -- H100-native (sm_90a CUDA) drop-in for ADflow's per-block
 residual / smoother / matrix-free Jacobian-vector hot path.
 
 Only what the path needs lives here: ``csrc/`` (CUDA kernels + the C ABI of

@@ -56,7 +56,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise AdflowB200Error(
-            "%s not found: build it with `python -m adflow_b200.build` (nvcc, sm_100a). "
+            "%s not found: build it with `python -m adflow_b200.build` (nvcc, sm_90a). "
             "There is no CPU fallback." % LIB_PATH
         )
     L = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)

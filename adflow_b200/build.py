@@ -1,4 +1,4 @@
-"""Build recipe for libadflow_b200.so (nvcc, sm_100a only, in-tree)."""
+"""Build recipe for libadflow_b200.so (nvcc, sm_90a only, in-tree)."""
 import os
 import subprocess
 import sys
@@ -8,14 +8,15 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libadflow_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
 ]
 
 
 def sources():
+    """everything the library depends on, this recipe included: a change of FLAGS (the target architecture) rebuilds it"""
     return [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh"))] + [
-        os.path.join(HERE, "..", "include", "adflow_b200.h")]
+        os.path.join(HERE, "..", "include", "adflow_b200.h"), os.path.abspath(__file__)]
 
 
 def stale():

@@ -453,8 +453,8 @@ int adfb_block_create(int blk, int level, int nx, int ny, int nz, int nw, int ri
     BlockDev& v = b.dev;
     memset(&v, 0, sizeof v);
     int rc = 0;
-    // state slab: w(nw), p, rlv, rev contiguous, so that one L2 access-policy window can keep the arrays every
-    // kernel of a step re-reads resident in the 126 MB L2 (set_l2_window below)
+    // state slab: w(nw), p, rlv, rev contiguous, so that one L2 access-policy window can cover the arrays every kernel of
+    // a step re-reads (set_l2_window below, off by default)
     rc |= dalloc(b, &v.w, N * (nw + 3));
     v.p = v.w + N * nw; v.rlv = v.p + N; v.rev = v.rlv + N;
     b.slabBytes = (size_t)N * (nw + 3) * sizeof(double);
@@ -1008,7 +1008,10 @@ int adfb_residual(int level, unsigned flags) {
 // nodes of captured graphs).  Only when exactly one block lives on the device (one window per stream).
 static void set_l2_window() {
     static int mode = -1;
-    if (mode < 0) { const char* e = getenv("ADFB_L2_PERSIST"); mode = e ? atoi(e) : 1; }
+    // Off by default: on H100 (50 MB L2) the C2 slab (37 MB) takes most of the persisting set-aside and starves the streamed
+    // arrays.  C2 on one H100 SXM (400 W limit): residual step 1396 Mcells/s off, 1177 on; 5-stage RK cycle 1.59 ms off,
+    // 2.58 ms on.  ADFB_L2_PERSIST=1 turns it on.
+    if (mode < 0) { const char* e = getenv("ADFB_L2_PERSIST"); mode = e ? atoi(e) : 0; }
     static const void* current = nullptr;
     Block* only = nullptr;
     int nAlive = 0;
@@ -1041,8 +1044,8 @@ static void set_l2_window() {
 static int residual_body(int level, unsigned flags) {
     // The inner part of k_prep and of the SA row read no halo cell, so they do not have to wait for the boundary conditions
     // and the exchange: with ADFB_OVERLAP_BC=1 they run on a second stream beside the BC chain and are joined before the
-    // halo-dependent rest.  Measured (round 2, C2): 0.315 vs 0.287 ms per step -- the small dependent BC launches queue
-    // behind the big kernels' CTAs and the chain gets longer than the work it hides; off by default.
+    // halo-dependent rest.  The small dependent BC launches then queue behind the big kernels' CTAs and the chain gets
+    // longer than the work it hides; off by default.
     static int overlapOn = -1;
     if (overlapOn < 0) { const char* e = getenv("ADFB_OVERLAP_BC"); overlapOn = e ? atoi(e) : 0; }
     static cudaStream_t s2 = nullptr;
@@ -1174,7 +1177,7 @@ static bool ff_pinned(const void* p) {
 }
 static int form_function_pipe_slabs() {   // read at every call: tests switch it
     const char* e = getenv("ADFB_FF_PIPE");
-    return e ? atoi(e) : 6;   // C2, final tile kernel: 6 slabs 0.660 ms, 8 slabs 0.694 ms, 10 slabs 0.696 ms per call
+    return e ? atoi(e) : 6;   // C2 on one H100 SXM (400 W limit): 4 / 6 / 8 / 12 slabs 0.87 / 0.75 / 0.78 / 0.74 ms per call
 }
 // the stream work of one pipelined call (captured into a CUDA graph per (wVec, rVec) pair: ~15 launches per slab otherwise
 // cost more host time than the GPU needs for them).  Front end of a slab (setW, p / rlv / rev, BCs, time step / sensor) on the
@@ -1409,9 +1412,9 @@ static int mffd_core(long long need, double h) {
     // the owned cells, and the kernels that write dw (tile kernel, k_sa) form y = (R - F0) / h of their rows; bitwise
     // the unfused product (same operations on the same operands).  ADFB_MFFD_FUSED=0, or a block the tile kernel does not
     // take (matrix / upwind dissipation, coarse level), selects the three-pass form.
-    // Measured on C2 (round 2): 0.367 ms fused against 0.361 ms in three passes -- the two extra vector passes cost less
-    // than the strided AoS accesses of the epilogue inside the tile kernel, the product is not bandwidth bound.  The
-    // three-pass form therefore stays the default; ADFB_MFFD_FUSED=1 selects the fused one.
+    // The two extra vector passes of the three-pass form cost less than the strided AoS accesses of the epilogue inside
+    // the tile kernel (the product is not bandwidth bound), so the three-pass form stays the default; ADFB_MFFD_FUSED=1
+    // selects the fused one.
     bool fuse = false;
     { const char* e = getenv("ADFB_MFFD_FUSED"); if (e && e[0] == '1') fuse = true; }
     if (g_kt.on) fuse = false;

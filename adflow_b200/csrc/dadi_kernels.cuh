@@ -306,7 +306,7 @@ __global__ void __launch_bounds__(64) k_dadi_thomas(Dims d, BlockDev b, int sd, 
 // with the arithmetic of the previous one (12 dependent round trips per sweep on a 96-cell line), (2) for lines along i
 // (sd == 1), where neighbouring THREADS own lines a whole row apart, the lanes copy along the line (8 consecutive cells =
 // one 64-byte segment per 8 lanes) instead of touching 32 cache lines per load instruction -- that sweep was bound by L1
-// wavefronts (79 us against 28 us for the other two directions on C2).  Same operations on the same operands.
+// wavefronts.  Same operations on the same operands.
 #define ADFB_DT_CH 8
 #define ADFB_DT_WARPS 4
 struct DtSmem {
@@ -561,8 +561,8 @@ static int launch_dadi(const Dims& d, const BlockDev& b, const AdfbParams& prm, 
     // (a partitioned, 8-lanes-per-line variant of this solve was measured slower here: with 5 systems per line the
     // serial walks already fill the machine and the partition method does 2.5x the arithmetic; it pays for the
     // single-system SA solve only, see sa_kernels.cuh)
-    // ADFB_DADI_SMEM=1: rows + solve in shared memory (k_dadi_lines; parity-clean, measured slower on C2 than k_dadi_tri + the
-    // thread-per-(line, variable) walks: 0.43 vs 0.35 ms per step -- 14 arrays per line leave 16 lines per CTA and two waves)
+    // ADFB_DADI_SMEM=1: rows + solve in shared memory (k_dadi_lines; parity-clean, slower on C2 than k_dadi_tri + the
+    // thread-per-(line, variable) walks: 14 arrays per line leave 16 lines per CTA and two waves)
     static int smemLines = -1;
     if (smemLines < 0) { const char* e = getenv("ADFB_DADI_SMEM"); smemLines = e ? atoi(e) : 0; }
     auto lines_lpc = [&](int nl) {

@@ -1,4 +1,4 @@
-// fused_kernels.cuh -- k-marching tile kernel for the flow rows of the residual (sm_100a)
+// fused_kernels.cuh -- k-marching tile kernel for the flow rows of the residual (sm_90a)
 //
 // One launch replaces k_nodal -> k_faces -> k_div of residual_kernels.cuh for the exact
 // central + scalar-JST (+ viscous) residual, i.e. the reference's own tiled formulation
@@ -40,9 +40,10 @@
 #endif
 
 #ifndef FT_MAXT
-#define FT_MAXT 256   // max threads per CTA of the tile kernel (1 CTA / SM; 252 registers, no spills; final tree on C2: 117 us with the
-                      // 17 x 13 tile ftile_choose picks; 320 / 384 threads at 168 registers spill: 171 / 161 us; two CTAs of 128
-                      // threads per SM (-DFT_MAXT=128 -DFT_S2=224 -DFT_MINB=2) 111 us)
+#define FT_MAXT 256   // max threads per CTA of the tile kernel (1 CTA / SM).  sm_90a, ptxas: 255 registers, the merged viscous kernel
+                      // spills 64 B (stores) / 96 B (loads), the split one 132 / 204 B.  Two CTAs of 128 threads per SM
+                      // (-DFT_MAXT=128 -DFT_S2=224 -DFT_MINB=2) get the same 255 registers and run the C2 step at 1065 against
+                      // 1177 Mcells/s (one H100 SXM, 400 W limit, L2 window on)
 #endif
 
 // ring variables (shared-memory state tiles)
@@ -667,11 +668,12 @@ FHD bool ft_var_used(int v, bool viscous, int doDiss) {
 #define FT_EARLY 0
 #endif
 // FT_AHEAD (bits): 1 / 2 = the operands of the j / k face are requested before the i face is formed (their L2 latency hides
-// behind its arithmetic; 242-254 registers, no spills: 134 -> 128 us on C2, default 3); 4 = the nodal operands of the next plane at
-// the end of the step (spills 60 bytes: 138 us, off); 8 = the i-face operands before the barrier that follows the nodal phase
-// (129.5 us with 3: no gain, off)
+// behind its arithmetic); 4 = the nodal operands of the next plane at the end of the step; 8 = the i-face operands before the
+// barrier that follows the nodal phase.  On sm_90a every setting runs at the 255-register cap and the requests ahead cost spills
+// (merged kernel, ptxas: 0 -> 64 B, 1 -> 100 B, 2 -> 96 B, 3 -> 140 B of spill stores).  C2 on one H100 SXM (400 W limit), tile
+// kernel / residual step: 0 -> 154 us / 1396 Mcells/s, 1 -> 165 / 1358, 2 -> 171 / 1370, 3 -> 172 / 1317; default 0
 #ifndef FT_AHEAD
-#define FT_AHEAD 3
+#define FT_AHEAD 0
 #endif
 template <bool VISCOUS, bool MERGED>
 FHD void ft_step_a(const Dims& d, const BlockDev& b, const FTile& t, const FCtx& x, int k, int kb, const double* A, const double* B, FSmem& sm,
@@ -757,10 +759,11 @@ static inline bool ftile_fits(const FTile& t) { return t.nT <= FT_MAXT && t.PX *
 static inline FTile ftile_choose(const Dims& d, bool tma, int nSM) {
     int ox = 0, oy = 0, okc = 0;
     if (const char* e = getenv("ADFB_TILE")) sscanf(e, "%d,%d,%d", &ox, &oy, &okc);
-    // One CTA per SM, and the time of a k plane grows with the warps of the CTA (the kernel is issue bound inside the CTA): measured
-    // 2.3 + 0.69 x warps [us] per plane.  The cost of a choice is waves x (planes per chunk + the prologue step, ~0.45 of a plane) x that
-    // time; on C2: 13 x 19 threads, 5-plane chunks (3 waves of 8 warps) model 127.9 / measured 128.1 us; 17 x 13 threads, 16-plane chunks
-    // (1 wave of 7 warps) 117.3 / 117.5 us; the same tile with 8-plane chunks (2 waves) 120.5 / 122.4 us.
+    // One CTA per SM, and the time of a k plane grows with the warps of the CTA (the kernel is issue bound inside the CTA): modelled
+    // as 2.3 + 0.69 x warps per plane (relative units).  The cost of a choice is waves x (planes per chunk + the prologue step, ~0.45
+    // of a plane) x that time.  The SM count is the device's, so the pick follows the part: on one H100 SXM (132 SMs, 400 W limit)
+    // the C2 residual step runs at 1401 Mcells/s with the pick, against 1072-1260 with fixed ADFB_TILE choices (17,13,16 13,19,5
+    // 15,15,8 11,17,8 19,11,16).
     FTile best = ftile_make(tma ? 9 : 8, 4, d.nz, tma);
     double bestCost = 1e300;
     for (int pass = 0; pass < 2 && bestCost >= 1e300; pass++) {   // pass 0 honours ADFB_TILE, pass 1 (override does not fit) searches freely

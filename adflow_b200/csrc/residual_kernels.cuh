@@ -1,4 +1,4 @@
-// residual_kernels.cuh -- residual kernels (face-flux form) for sm_100a
+// residual_kernels.cuh -- residual kernels (face-flux form) for sm_90a
 //
 // Replaces the per-block residual core of the reference
 // (blocketteResCore, src/NKSolver/blockette.F90:299-753 and its operator twins in
@@ -27,7 +27,7 @@
 #include "fused_kernels.cuh"
 #include "geom_cell.cuh"
 
-// tunables (see profiles/): threads per block / min resident blocks per SM
+// tunables: threads per block / min resident blocks per SM
 #ifndef FACES_TPB
 #define FACES_TPB 128
 #endif
@@ -919,8 +919,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     if (!(parts & RC_FLOW)) return (int)cudaGetLastError();
     bool fusedDone = false;
     // (smoother path, persistFw: the tile kernel exchanges central and dissipative fluxes separately with two more CTA
-    // barriers per plane and measured slower than k_nodal/k_faces/k_div there: 1.37 vs 1.28 ms per RK cycle; ADFB_FUSED_SMOOTHER=1
-    // selects it anyway)
+    // barriers per plane and was slower than k_nodal/k_faces/k_div there; ADFB_FUSED_SMOOTHER=1 selects it anyway)
     static int fusedSmoother = -1;
     if (fusedSmoother < 0) { const char* e = getenv("ADFB_FUSED_SMOOTHER"); fusedSmoother = e ? atoi(e) : 0; }
     // ADFB_FUSED_SMOOTHER: 1 = the tile kernel for every smoother residual, 2 = only for the stages that form the dissipative and viscous

@@ -454,7 +454,7 @@ __global__ void __launch_bounds__(256) k_bc_frame(Dims d, BlockDev b, const BcLi
 // The whole ordered BC sweep of a block in ONE launch.  The reference applies the subfaces one after the other
 // (applyAllTurbBCThisBlock, then applyAllBC_block in its BC-class order, BCRoutines.F90:81-216), and the edge / corner
 // halos depend on that order, so the items stay strictly ordered -- but the hand-over from one item to the next is a
-// device-side counter instead of a kernel boundary (~6 us per dependent launch inside a graph): a CTA draws a ticket,
+// device-side counter instead of a kernel boundary (a dependent launch inside a graph): a CTA draws a ticket,
 // which names its item and its 32 x 4 patch of the subface, waits until every CTA of all earlier items has finished
 // (tickets are handed out in start order, so everything a CTA waits for is already running: no deadlock whatever the
 // dispatch order), applies the BC, and publishes its completion.
@@ -971,12 +971,10 @@ __global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev
 // ADFB_BC_FUSED: 5 = the whole sweep in one launch, exact (k_bc_sweep: bulk cells by all CTAs, the ordered frames by CTA 0);
 // 6 = the same with the frames walked by a cluster of 8 CTAs (k_bc_sweep_cluster);
 // 4 = one launch per LEVEL of mutually independent items (k_bc_level); 0 = one launch per subface and phase over all of its cells, chained by programmatic dependent
-// launch (13 launches of ~5 us for the bench block); 3 = the whole ordered sweep in one launch, items ordered by a device-side
-// counter (k_bc_chain: parity-clean, but the ticket / fence / counter hand-over costs 5.3 us per item, measured 69 us per sweep
-// against 65 us for the launch chain); 1 = one launch for the
-// order-independent cells of all subfaces, then the ordered frame items as small launches (round 2: 14 launches of
-// ~6 us each inside the graph, slower than 13 and not parity-clean: experiment only); 2 = bulk launch + one CTA
-// walking the frame items (measured slower in round 1)
+// launch (13 launches for the bench block); 3 = the whole ordered sweep in one launch, items ordered by a device-side
+// counter (k_bc_chain: parity-clean, but the ticket / fence / counter hand-over per item costs more than the launch chain);
+// 1 = one launch for the order-independent cells of all subfaces, then the ordered frame items as small launches (14 launches,
+// not parity-clean: experiment only); 2 = bulk launch + one CTA walking the frame items (slower)
 static int bc_mode() {
     static int v = -1;
     if (v < 0) { const char* e = getenv("ADFB_BC_FUSED"); v = e ? atoi(e) : 4; }

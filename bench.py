@@ -41,14 +41,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 C2 = (96, 72, 64)
-# DRAM traffic of one residual step on C2 measured by ncu (profiles/r02_ncu_summary.md: sum over the four residual kernels
-# k_state_prep + k_sa + k_prep + k_flowres; round 1 had 568.1e6 over six kernels)
-NCU_TRAFFIC_BYTES = 403.6e6
-NCU_TRAFFIC_NOTE = ("dram__bytes_read.sum + dram__bytes_write.sum summed over the residual kernels of one step, ncu --set full capture "
-                    "(profiles/)")
 # the second roof (SURVEY section 7 'report both'): the path is FP64-issue bound long before it is HBM bound
-FP64_ROOF = {"note": "B200 FP64 pipe: 64 DFMA lanes / SM / clk x 148 SMs x 1.965 GHz = 18.6 T FP64 instructions/s (37 TFLOP/s); "
-                     "percentages of the dominant kernel k_flowres from the ncu --set full capture profiles/r02_ncu_summary.md", "fp64_pipe_pct": 23.9, "issue_active_pct": 27.9}
+FP64_ROOF = {"note": "H100 SXM FP64 pipe (data sheet, 700 W): 64 DFMA lanes / SM / clk x 132 SMs x 1.98 GHz = 16.7 T FP64 "
+                     "instructions/s (33.5 TFLOP/s); the pipe utilisation of the kernels is not measured"}
 BYTES_PER_CELL = 176.0  # SURVEY.md 8(d): RANS-SA residual, metrics from x, algorithmic
 METRIC = "Mcells/s RANS-SA residual"
 
@@ -58,7 +53,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -255,6 +250,29 @@ def run_reference(args):
     return 0
 
 
+DUMP_BYTES = 64 << 20
+NPY_HEADER_MAX = 256   # bytes; an .npy header of a 1- or 2-d float64 array is 128
+
+
+def dump_outputs(out_dir, s, blocks, rank, world, np):
+    """What the timed step hands its caller: dw of the owned cells of every local block (float64, (nx, ny, nz, nw)) and
+    the two residual norms.  Where all ranks' dw together exceed DUMP_BYTES, each block is cut to the same seeded sample
+    of cells (flattened in Fortran order), so that runs with the same arguments write comparable files."""
+    os.makedirs(out_dir, exist_ok=True)
+    tag = "" if world == 1 else "rank%d_" % rank
+    # every rank writes one file per block and one norms file (16 bytes of data): reserve their headers
+    per_block = (DUMP_BYTES - world * (NPY_HEADER_MAX * (len(blocks) + 1) + 16)) // (world * len(blocks))
+    for q, hb in enumerate(blocks):
+        dw = np.asfortranarray(s.downloadResidual(q)[hb.d.owned()])
+        if dw.nbytes > per_block:
+            flat = dw.reshape(-1, dw.shape[-1], order="F")
+            keep = per_block // (8 * flat.shape[1])
+            pick = np.sort(np.random.default_rng(2718).choice(flat.shape[0], keep, replace=False))
+            dw = flat[pick]
+        np.save(os.path.join(out_dir, "%sdw_block%d.npy" % (tag, q)), np.ascontiguousarray(dw, dtype=np.float64))
+    np.save(os.path.join(out_dir, "%sres_norms.npy" % tag), np.asarray(s.getResNorms(), dtype=np.float64))
+
+
 def workload_name(shape, nblocks):
     return "C2 %dx%dx%d RANS-SA residual (blocketteRes), %d block(s)" % (tuple(shape) + (nblocks,))
 
@@ -339,7 +357,7 @@ def halo_data_check(s, blocks, pat, np, torch=None, dist=None):
 # residual norms of the C3 8-block case after one 5-stage RK cycle from the synthetic state, measured at N = 1 (all
 # eight blocks on one GPU): every other distribution of the same blocks must reproduce them (partition independence,
 # the reference's analogue: tests/reg_tests/test_functionals.py:24-58).  None = not recorded yet.
-C3_REF_NORMS = (1233939870.9755895, 26154234242.979332)   # measured at N = 1 (8 blocks on one B200), round 2
+C3_REF_NORMS = (1233939870.9755895, 26154234242.979332)   # computed at N = 1 (8 blocks on one GPU)
 
 
 def strong_scaling_c3(args, torch, dist, rank, world, local, fresh_uid, np):
@@ -464,6 +482,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--shape", type=int, nargs=3, default=list(C2))
     ap.add_argument("--no-scaling-sections", action="store_true", help="skip the C3 strong-scaling and C5 matvec sections")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the residual of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -551,6 +570,8 @@ def main():
     ms_total = timed_steps(step, args.steps)
     launches = s.launchCount() - n0
     barrier()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, s, blocks, rank, world, np)
     # ---- e2e through the vector API with pinned host buffers -------------------
     nvec = s.getStateSize()
     h_state = torch.empty(nvec, dtype=torch.float64).pin_memory()
@@ -584,7 +605,7 @@ def main():
     res_three = h_res.numpy().copy()
     e2e_ms = wall_ms(e2e_step)
     e2e_maxdiff = float(np.abs(h_res.numpy() - res_three).max() / max(np.abs(res_three).max(), 1e-300))
-    # nvidia-smi answers every 100 ms and needs a few hundred ms for its first line; a short timed region (K steps of 0.3 ms) can end
+    # nvidia-smi answers every 100 ms and needs a few hundred ms for its first line; a short timed region (K steps of a fraction of a ms) can end
     # before it.  The same step keeps running, untimed, for a fixed number of launches on every rank (the step holds a collective
     # at N > 1), so that the clocks and throttle reasons reported are those of this workload under load.
     for _ in range(60):
@@ -773,8 +794,6 @@ def main():
                          "frac_from_step_time": BYTES_PER_CELL * cells / (ms_step * 1e-3) / 1e9 / peak,
                          "frac_note": "frac: 176 B/cell x cells / SUM of the per-kernel event times of one step (separate timing pass, "
                                       "side-stream overlap counted twice: conservative); frac_from_step_time: same bytes / ms_per_step",
-                         "traffic": NCU_TRAFFIC_BYTES if tuple(shape) == tuple(C2) else None,
-                         "traffic_note": NCU_TRAFFIC_NOTE,
                          "peak_source": peak_src,
                          "kernel": "whole residual step: all launches (state prep, BCs, halo pack/unpack, k_prep, k_flowres tile kernel, "
                                    "k_sa) charged against 176 B/cell",
@@ -783,7 +802,7 @@ def main():
                              "name": dom[0], "ms_per_launch": dom[1]["ms_per_launch"],
                              "share_of_summed_kernel_time": dom[1]["ms_per_launch"] * dom[1]["launches"] / (res_ms * args.steps),
                              "GB/s_if_charged_the_whole_176_B_per_cell": BYTES_PER_CELL * cells / (dom[1]["ms_per_launch"] * 1e-3) / 1e9,
-                             "note": "the tile kernel k_flowres (flow rows of the residual); its own ncu numbers are in profiles/r02_ncu_summary.md"},
+                             "note": "the tile kernel k_flowres (flow rows of the residual)"},
                          "second_roof": FP64_ROOF},
             "clocks": clocks,
         }

@@ -1,7 +1,7 @@
 /*
  * adflow_b200.h -- C ABI of libadflow_b200.so
  *
- * B200-native (sm_100a) implementation of the per-block residual / smoother /
+ * H100-native (sm_90a) implementation of the per-block residual / smoother /
  * matrix-free Jacobian-vector hot path of mdolab/adflow.  The reference has no
  * FFI seam around this path (SURVEY.md section 8b): its L2 routines are
  * argument-less Fortran module procedures acting on module-global block
