@@ -124,3 +124,62 @@ def test_emulated_tile_kernel_smoother_path(rfil, do_diss):
     for l in range(5):
         assert rel_l2(dw[ow + (l,)], h2.dw[ow + (l,)]) < 1e-12, l
         assert rel_l2(fw[ow + (l,)], h2.fw[ow + (l,)]) < 1e-12, l
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# flow regimes the smooth state never reaches (tests/regimes.py): a contact discontinuity caps the JST sensor at 0.25
+# and cuts the fourth difference off on its faces.  The tile kernel forms i and j faces in shared memory and k faces in
+# registers, so each direction is checked, with the jump inside a tile, on a tile seam (the face between the last
+# owned cell of one tile and the first of the next: box index 2 + (T-1)) and one cell past it; for k on a chunk seam.
+TILE = (9, 5, 4)
+SEAMS = {"contact_i": [2 + (TILE[0] - 1) // 2, 2 + TILE[0] - 1, 3 + TILE[0] - 1],
+         "contact_j": [2 + (TILE[1] - 1) // 2, 2 + TILE[1] - 1, 3 + TILE[1] - 1],
+         "contact_k": [2 + TILE[2] // 2, 2 + TILE[2], 3 + TILE[2]]}
+
+
+def _regime_rows_close(hb, regime, at, got, want, tol=1e-12):
+    import regimes as R
+
+    ow = hb.d.owned()
+    far = None if regime == "supersonic" else R.owned_away_from(hb, regime, at)
+    for l in range(5):
+        a, b = got[ow + (l,)], want[ow + (l,)]
+        assert np.isfinite(a).all(), l
+        assert rel_l2(a, b) < tol, (l, rel_l2(a, b))
+        if far is not None:    # a jump cell's residual can dwarf the rest: hold the cells away from it on their own
+            assert rel_l2(a[far], b[far]) < tol, ("away from the jump", l, rel_l2(a[far], b[far]))
+
+
+REGIME_CASES = [(r, at) for r in ("contact_i", "contact_j", "contact_k") for at in SEAMS[r]] + [("supersonic", None)]
+
+
+@pytest.mark.parametrize("regime,at", REGIME_CASES)
+def test_emulated_tile_kernel_in_regimes(regime, at):
+    import regimes as R
+    from test_regimes_reach import assert_reaches
+
+    prm, hb = R.regime_case(regime, (12, 10, 8), at=at)
+    assert_reaches(prm, hb, regime, ["sensor_cap_" + a for a in ("ijk" if regime == "supersonic" else regime[-1])])
+    ho = oracle_residual(prm, hb, FLOW | TURB)
+    dw, _ = run_emul(prm, hb, ho, *TILE)
+    _regime_rows_close(hb, regime, at, dw, ho.dw)
+
+
+@pytest.mark.parametrize("regime,at", REGIME_CASES)
+def test_emulated_smoother_path_in_regimes(regime, at):
+    """merged = 0, persistent fw (the RK / DADI block path) with rFil 0.56: the blend of the capped dissipation"""
+    import regimes as R
+    from oracle.pyoracle import Oracle
+
+    prm, hb = R.regime_case(regime, (12, 10, 8), at=at)
+    h2 = hb.copy()
+    o = Oracle(h2, prm)
+    o.time_step(True)
+    h2.fw[...] = np.random.default_rng(1).standard_normal(h2.fw.shape) * 1e-3
+    fw0 = h2.fw.copy()
+    o.residual_block(0.56)
+    hs = oracle_residual(prm, hb, FLOW | TURB)
+    hs.radI[...], hs.radJ[...], hs.radK[...] = h2.radI, h2.radJ, h2.radK
+    dw, fw = run_emul(prm, hb, hs, *TILE, rfil=0.56, do_diss=1, merged=0, persist_fw=1, fw=fw0)
+    _regime_rows_close(hb, regime, at, dw, h2.dw)
+    _regime_rows_close(hb, regime, at, fw, h2.fw)

@@ -79,7 +79,7 @@ def test_general_kernels_still_match(cuda_lib):
     env = dict(os.environ, ADFB_FUSED="0")
     here = os.path.dirname(os.path.abspath(__file__))
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(here, "test_residual_parity.py"), os.path.join(here, "test_cuda_vs_reference.py"),
-                        os.path.join(here, "test_smoother_parity.py"), "-m", "gpu", "-q", "-x"], env=env, capture_output=True, text=True, timeout=900)
+                        os.path.join(here, "test_smoother_parity.py"), os.path.join(here, "test_regimes_gpu.py"), "-m", "gpu", "-q", "-x"], env=env, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
 
 
