@@ -866,7 +866,8 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     const bool viscous = prm.equations != ADFB_EULER;
     const int doDiss = fabs(rFil) >= 1.e-10;  // fluxes.F90:1082 early return
     const int doVisc = viscous && doDiss;
-    const int dissApprox = (flags & ADFB_RES_DISS_APPROX) ? 1 : 0, viscApprox = (flags & ADFB_RES_VISC_APPROX) ? 1 : 0;
+    // useViscApprox only selects the thin-layer viscous flux (blockette.F90:636-644): an inviscid block ignores it
+    const int dissApprox = (flags & ADFB_RES_DISS_APPROX) ? 1 : 0, viscApprox = (viscous && (flags & ADFB_RES_VISC_APPROX)) ? 1 : 0;
     if ((dissApprox || viscApprox) && persistFw) return 1;  // approximate variants exist on the blockette path only
     // experiment switch: AoS nodal-gradient store, only for the exact merged viscous scalar-JST residual (the bench path)
     const bool gradAos = grad_aos() && flowRes && doVisc && !persistFw && !dissApprox && !viscApprox && !b.coarse && !split_faces() &&

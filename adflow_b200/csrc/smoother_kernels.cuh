@@ -346,15 +346,20 @@ __global__ void __launch_bounds__(128) k_bc_flow(Dims d, BlockDev b, FaceDev f, 
 
 // ---------------------------------------------------------------------------
 // All BCs of a block in TWO launches.  The order in which applyAllBC_block / applyAllTurbBCThisBlock visit the
-// subfaces only matters where subfaces share halo cells: the frame of every subface (in-plane index outside the owned
-// range 2:l, i.e. the edge and corner halos).  Face cells with owned in-plane indices read owned cells and write halo
-// cells no other subface touches, so
-//   k_bc_bulk  : those cells of ALL subfaces at once (turbulence BC, then the flow BC incl. both symmetry phases), and
-//   k_bc_frame : the frames, one CTA walking the reference's ordered list of (subface, phase) items with a barrier
-//                between items (a frame has 2(na+nb) cells).
-// A frame cell may read a bulk halo cell of a subface that comes LATER in the reference's order (there: the old value);
-// every such cell is written again by that later subface's own frame item, which reads the earlier subface's bulk
-// cells -- already updated in the reference as well -- so the final halo values are the reference's.
+// subfaces only matters where subfaces touch common cells.  A face cell (a, b) reads the two owned cells and writes the
+// two halo cells of its own grid line, so it can only meet a subface of an adjacent face when one of its in-plane indices
+// lies within three cells of that face (indices 0..3 or l-1..l+1, see k_bc_sweep below).  So
+//   k_bc_bulk  : the cells with in-plane indices 4 .. l-2 of ALL subfaces at once (turbulence BC, then the flow BC incl.
+//                both symmetry phases): no other subface reads or writes their cells, any order is the reference's, and
+//   k_bc_frame : the rest of every subface (three layers along each block edge), one CTA walking the reference's ordered
+//                list of (subface, phase) items with a barrier between items.
+// (The whole owned range 2 .. l is NOT conflict-free: a frame cell of one subface reads the halo that an adjacent subface
+// later in the reference's order writes from its owned-range cells.)
+__device__ __forceinline__ void bc_bulk_box(const FaceDev& f, int la, int lb, int* a0, int* a1, int* b0, int* b1) {
+    *a0 = f.icBeg > 4 ? f.icBeg : 4; *a1 = f.icEnd < la - 2 ? f.icEnd : la - 2;
+    *b0 = f.jcBeg > 4 ? f.jcBeg : 4; *b1 = f.jcEnd < lb - 2 ? f.jcEnd : lb - 2;
+    if (*a1 < *a0 || *b1 < *b0) { *a0 = f.icBeg; *a1 = f.icEnd; *b0 = f.jcEnd + 1; *b1 = f.jcEnd; }   // no bulk: all rows are frame
+}
 #define ADFB_BC_MAXSUB 12
 struct BcList {
     int n;
@@ -387,8 +392,8 @@ __global__ void __launch_bounds__(128) k_bc_bulk(Dims d, BlockDev b, const BcLis
     const BcList& L = *Lp;
     const int s = blockIdx.z;
     const FaceDev& f = L.f[s];
-    const int a0 = f.icBeg > 2 ? f.icBeg : 2, a1 = f.icEnd < L.la[s] ? f.icEnd : L.la[s];
-    const int b0 = f.jcBeg > 2 ? f.jcBeg : 2, b1 = f.jcEnd < L.lb[s] ? f.jcEnd : L.lb[s];
+    int a0, a1, b0, b1;
+    bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
     const int ia = blockIdx.x * blockDim.x + threadIdx.x + a0;
     const int jb = blockIdx.y * blockDim.y + threadIdx.y + b0;
     if (ia > a1 || jb > b1) return;
@@ -439,8 +444,8 @@ __global__ void __launch_bounds__(256) k_bc_frame(Dims d, BlockDev b, const BcLi
     for (int it = 0; it < nItems; it++) {
         const int s = itemS[it], kind = itemK[it];
         const FaceDev& f = L.f[s];
-        const int a0 = f.icBeg > 2 ? f.icBeg : 2, a1 = f.icEnd < L.la[s] ? f.icEnd : L.la[s];
-        const int b0 = f.jcBeg > 2 ? f.jcBeg : 2, b1 = f.jcEnd < L.lb[s] ? f.jcEnd : L.lb[s];
+        int a0, a1, b0, b1;
+        bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
         for (int q = threadIdx.x;; q += blockDim.x) {
             int ia, jb;
             if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) break;
@@ -504,8 +509,8 @@ __global__ void __launch_bounds__(128) k_bc_frame_item(Dims d, BlockDev b, const
     ADFB_PDL_SYNC();
     const BcList& L = *Lp;
     const FaceDev& f = L.f[s];
-    const int a0 = f.icBeg > 2 ? f.icBeg : 2, a1 = f.icEnd < L.la[s] ? f.icEnd : L.la[s];
-    const int b0 = f.jcBeg > 2 ? f.jcBeg : 2, b1 = f.jcEnd < L.lb[s] ? f.jcEnd : L.lb[s];
+    int a0, a1, b0, b1;
+    bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
     int ia, jb;
     if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) return;
@@ -553,11 +558,6 @@ struct BcSweep {
     int nSub, la[ADFB_BC_MAXSUB], lb[ADFB_BC_MAXSUB];       // by value (constant bank): no dependent global load before the state loads
     FaceDev f[ADFB_BC_MAXSUB];
 };
-__device__ __forceinline__ void bc_bulk_box(const FaceDev& f, int la, int lb, int* a0, int* a1, int* b0, int* b1) {
-    *a0 = f.icBeg > 4 ? f.icBeg : 4; *a1 = f.icEnd < la - 2 ? f.icEnd : la - 2;
-    *b0 = f.jcBeg > 4 ? f.jcBeg : 4; *b1 = f.jcEnd < lb - 2 ? f.jcEnd : lb - 2;
-    if (*a1 < *a0 || *b1 < *b0) { *a0 = f.icBeg; *a1 = f.icEnd; *b0 = f.jcEnd + 1; *b1 = f.jcEnd; }   // no bulk: all rows are frame
-}
 __global__ void __launch_bounds__(512) k_bc_sweep(Dims d, BlockDev b, const BcList* __restrict__ Lp, const __grid_constant__ BcSweep sw, int secondHalo, int withTurb,
                                                   int withFlow) {
     ADFB_PDL_SYNC();
@@ -973,8 +973,9 @@ __global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev
 // 4 = one launch per LEVEL of mutually independent items (k_bc_level); 0 = one launch per subface and phase over all of its cells, chained by programmatic dependent
 // launch (13 launches for the bench block); 3 = the whole ordered sweep in one launch, items ordered by a device-side
 // counter (k_bc_chain: parity-clean, but the ticket / fence / counter hand-over per item costs more than the launch chain);
-// 1 = one launch for the order-independent cells of all subfaces, then the ordered frame items as small launches (14 launches,
-// not parity-clean: experiment only); 2 = bulk launch + one CTA walking the frame items (slower)
+// 1 = one launch for the order-independent cells of all subfaces (k_bc_bulk), then the ordered frame items as small launches
+// (k_bc_frame_item, 14 launches); 2 = the same bulk launch + one CTA walking the frame items (k_bc_frame, slower).  All of them
+// are exact: tests/kernel_table.py runs the BC parity tests under each mode.
 static int bc_mode() {
     static int v = -1;
     if (v < 0) { const char* e = getenv("ADFB_BC_FUSED"); v = e ? atoi(e) : 4; }
@@ -1162,7 +1163,7 @@ static int launch_bc_fused(const Dims& d, const BlockDev& b, const std::vector<A
     auto item = [&](int q, int kind) {
         const AdfbSubface& sf = subs[q];
         const int na = sf.icEnd - sf.icBeg + 1, nb = sf.jcEnd - sf.jcBeg + 1;
-        const int nFrame = 2 * (na + nb);   // upper bound of the frame cells of one subface (frame_cell() rejects the rest)
+        const int nFrame = na * nb;   // upper bound of the frame cells of one subface (frame_cell() rejects the rest)
         KT_BEGIN(K_BC, s);
         launch_pdl(k_bc_frame_item, dim3((nFrame + 127) / 128), dim3(128), s, d, b, L, q, kind, secondHalo);
         KT_END(K_BC, s);

@@ -58,7 +58,8 @@ def oracle_ank_function(prm, ank, hb, T, vec):
 
 
 @pytest.mark.parametrize("options,coupled,kind,fullvisc", [(None, False, "None", True), (None, True, "None", False),
-                                                          (None, False, "VLR", True), ({"equationType": "Euler"}, False, "Turkel", True)])
+                                                          (None, False, "VLR", True), ({"equationType": "Euler"}, False, "Turkel", True),
+                                                          (None, True, "VLR", True), (None, True, "Turkel", False)])
 def test_ank_operator_and_product(cuda_lib, options, coupled, kind, fullvisc):
     prm, hb = case(11, 9, 8, options)
     ank = make_ank_params(cfl=5.0, coupled=coupled, char_time_step=kind, mach=0.8, cflLimit=50.0, turbCFLScale=2.0, useFullVisc=fullvisc)
@@ -157,12 +158,14 @@ def _host_gmres(apply, b, restart, max_its, rtol):
     return x, its
 
 
-@pytest.mark.parametrize("kind,coupled", [("None", False), ("VLR", True)])
-def test_device_gmres_on_a_linear_operator(cuda_lib, kind, coupled):
+@pytest.mark.parametrize("kind,coupled,shape", [("None", False, (9, 8, 7)), ("VLR", True, (9, 8, 7)),
+                                               ("VLR", True, (40, 32, 16))],   # n = 122 880: the 256 CTAs of the dot products loop
+                         ids=["None-False", "VLR-True", "VLR-True-large"])
+def test_device_gmres_on_a_linear_operator(cuda_lib, kind, coupled, shape):
     """adfb_gmres_solve on the block-diagonal time-step matrix (a LINEAR operator whose blocks the oracle provides):
     two restart cycles reproduce a host GMRES with the same parameters and the estimate of the recurrence is the true
     residual; with the exact inverse as right preconditioner (a callback on the device vectors) it converges at once"""
-    prm, hb = case(9, 8, 7)
+    prm, hb = case(*shape)
     ank = make_ank_params(cfl=3.0, coupled=coupled, char_time_step=kind, cflLimit=20.0, turbCFLScale=2.0)
     ns = hb.nw if coupled else 5
     o = Oracle(hb, prm)

@@ -55,6 +55,15 @@ def test_oracle_dadi_smoother_reduces_residual():
     (None, (20, 17, 16)),         # lines >= 16 cells: partitioned Thomas kernels (8 lanes per line)
     ({"resAveraging": "always", "CFL": 5.0}, (33, 18, 40)),
     ({"equationType": "Euler"}, (16, 35, 9)),   # mixed: i, j partitioned, k serial
+    ({"discretization": "central plus matrix dissipation", "equationType": "Euler"}, (12, 9, 10)),
+    ({"discretization": "upwind", "equationType": "laminar NS"}, (12, 9, 10)),
+    ({"discretization": "upwind"}, (12, 9, 10)),
+    # line lengths for each lines-per-CTA of the shared-memory solve (ADFB_DADI_SMEM=1, 14 arrays of nl (L + 1) doubles
+    # in 220 KiB): L = 32 up to 60 cells, 16 up to 118, 8 up to 223, 4 up to 402
+    (None, (60, 61, 4)),
+    (None, (118, 119, 3)),
+    (None, (223, 224, 2)),
+    ({"equationType": "Euler"}, (402, 7, 3)),
 ])
 def test_dadi_step_matches_oracle(cuda_lib, options, shape):
     prm, hb0 = case(*shape, options)

@@ -86,7 +86,9 @@ def prepare_fine(o):
 @pytest.mark.parametrize("shape,options", [((16, 12, 10), None), ((13, 9, 7), None), ((12, 8, 8), {"equationType": "Euler"}),
                                            ((10, 12, 6), {"equationType": "laminar NS"}),
                                            ((12, 10, 8), {"coarseDiscretization": "central plus matrix dissipation"}),
-                                           ((12, 10, 8), {"coarseDiscretization": "upwind"})])
+                                           ((12, 10, 8), {"coarseDiscretization": "upwind"}),
+                                           ((12, 10, 8), {"equationType": "Euler", "coarseDiscretization": "central plus matrix dissipation"}),
+                                           ((12, 10, 8), {"equationType": "Euler", "coarseDiscretization": "upwind"})])
 def test_restrict_smooth_prolong_match_oracle(cuda_lib, shape, options):
     prm, levels = make_levels(shape, options, 2)
     dev_levels = [l.copy() for l in levels]

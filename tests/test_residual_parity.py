@@ -9,7 +9,7 @@ import os
 import numpy as np
 import pytest
 
-from adflow_b200.solver import ADFLOW_B200, RES_FLOW, RES_SKIP_PREAMBLE, RES_TURB
+from adflow_b200.solver import ADFLOW_B200, RES_DISS_APPROX, RES_FLOW, RES_SKIP_PREAMBLE, RES_TURB, RES_VISC_APPROX
 
 from util import case, oracle_residual, rel_l2, rel_max
 
@@ -17,12 +17,15 @@ pytestmark = pytest.mark.gpu
 
 TOL = 1e-12
 GENERAL_KERNELS = os.environ.get("ADFB_FUSED") == "0"
+GRAD_AOS = os.environ.get("ADFB_GRAD_AOS", "0") != "0"
 
 
 def run_cuda(prm, hb, flags, upload_metrics=True):
     s = ADFLOW_B200(prm)
     try:
         s.addBlock(hb, upload_metrics=upload_metrics)
+        if flags & RES_DISS_APPROX:   # the approximate dissipation reads the frozen shock sensor
+            s.referenceShockSensor()
         s.residual(flags | RES_SKIP_PREAMBLE)
         dw = s.downloadResidual(0)
         inter = s.downloadIntermed(0)
@@ -66,7 +69,10 @@ def test_rans_sa_residual_matches_oracle(cuda_lib, shape):
     assert rel_max(extra["aa"][c1], ref.aa[c1]) < TOL
     if GENERAL_KERNELS:   # nodal gradients and shock sensor only exist in HBM on the general (k_nodal/k_faces/k_div) path
         nodes = (slice(1, d.il + 1), slice(1, d.jl + 1), slice(1, d.kl + 1))
-        assert rel_max(extra["grad"][nodes], ref.grad[nodes]) < TOL
+        grad = extra["grad"]
+        if GRAD_AOS:   # the 12 gradients of a node stored next to each other
+            grad = grad.ravel(order="F").reshape(-1, 12).reshape(grad.shape, order="F")
+        assert rel_max(grad[nodes], ref.grad[nodes]) < TOL
         assert rel_max(extra["dss"][c1], ref.dss[c1]) < 1e-9  # sensor is a ratio of small differences
 
 
@@ -103,6 +109,8 @@ def test_flow_only_and_turb_only(cuda_lib):
     {"discretization": "upwind", "limiter": "minmod"},
     {"discretization": "upwind", "limiter": "no limiter", "equationType": "laminar NS"},
     {"discretization": "upwind", "limiter": "first order", "equationType": "Euler"},
+    {"discretization": "upwind", "kappaCoef": -1.0},
+    {"discretization": "upwind", "kappaCoef": 0.0, "equationType": "laminar NS"},
 ])
 def test_option_variants(cuda_lib, options):
     prm, hb = case(14, 11, 10, options)
@@ -116,14 +124,44 @@ def test_metrics_computed_on_device(cuda_lib):
     compare(prm, hb, RES_FLOW | RES_TURB, upload_metrics=False)
 
 
-def test_porosity_and_iblank(cuda_lib):
-    prm, hb = case(12, 10, 8)
-    d = hb.d
+@pytest.mark.parametrize("upload_metrics", [False, True])
+def test_left_handed_block(cuda_lib, upload_metrics):
+    """x -> -x makes the block left handed: the face normals of `metrics` take the factor -0.5 instead of 0.5."""
+    from adflow_b200 import synthetic as syn
+    prm, hb = case(9, 8, 10)
+    hb.x[..., 0] *= -1.0
+    hb.right_handed = False
+    syn.compute_metrics(hb)
+    syn.compute_volumes(hb)
+    assert (hb.vol[hb.d.owned()] > 0).all()
+    compare(prm, hb, RES_FLOW | RES_TURB, upload_metrics=upload_metrics)
+
+
+def porosity_and_iblank_case(disc, approx):
+    prm, hb = case(12, 10, 8, {"discretization": disc})
     hb.porI[5, :, :] = -1   # noFlux plane
     hb.porJ[:, 4, :] = 0    # boundFlux plane
     hb.iblank[4:7, 4:6, 3:5] = 0
     hb.iblank[8, 8, 6] = -1
-    compare(prm, hb, RES_FLOW | RES_TURB)
+    if approx:
+        from oracle.pyoracle import Oracle
+        Oracle(hb, prm).reference_shock_sensor()
+        assert np.abs(hb.shock).max() > 0
+    compare(prm, hb, RES_FLOW | RES_TURB | (RES_DISS_APPROX | RES_VISC_APPROX if approx else 0))
+
+
+def test_porosity_and_iblank(cuda_lib):
+    porosity_and_iblank_case("central plus scalar dissipation", False)
+
+
+# the other discretisations, and all three with the approximate fluxes (scalar exact is test_porosity_and_iblank)
+POROSITY_VARIANTS = [(d, a) for d in ("scalar", "matrix", "upwind") for a in ("exact", "approx") if (d, a) != ("scalar", "exact")]
+DISCS = {"scalar": "central plus scalar dissipation", "matrix": "central plus matrix dissipation", "upwind": "upwind"}
+
+
+@pytest.mark.parametrize("disc,fluxes", POROSITY_VARIANTS, ids=["%s-%s" % c for c in POROSITY_VARIANTS])
+def test_porosity_and_iblank_variants(cuda_lib, disc, fluxes):
+    porosity_and_iblank_case(DISCS[disc], fluxes == "approx")
 
 
 def test_free_stream_preservation_on_device(cuda_lib):

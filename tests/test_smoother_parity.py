@@ -75,6 +75,9 @@ def test_full_residual_with_preamble(cuda_lib):
     {"equationType": "Euler", "nRKStages": 4, "resAveraging": "always", "CFL": 4.0},
     {"discretization": "central plus matrix dissipation", "nRKStages": 5, "resAveraging": "never"},
     {"discretization": "upwind", "equationType": "Euler", "nRKStages": 3, "resAveraging": "never"},
+    {"discretization": "central plus matrix dissipation", "equationType": "Euler", "nRKStages": 3, "resAveraging": "never"},
+    {"discretization": "upwind", "equationType": "laminar NS", "nRKStages": 5, "resAveraging": "never"},
+    {"discretization": "upwind", "nRKStages": 5, "resAveraging": "never"},
 ])
 def test_rk_cycle_matches_oracle(cuda_lib, options):
     prm, hb = case(16, 12, 10, options)
