@@ -62,7 +62,7 @@ struct BlockDev {
     // eddy viscosity, first-order dissipation: the currentLevel > groundLevel branches of the reference)
     double *wr, *w1, *p1;
     int coarse;
-    const void* bcList;   // device-resident BcList (smoother_kernels.cuh) of the block's subfaces, or null
+    const void* bcList;   // device-resident BcList (smoother_kernels.cuh) of the block's subfaces for k_sa_bmt_all, or null
 };
 
 // Matrix-free product fused into the residual (NKSolvers.F90:437-461 with setW :1331 and setRVec :1262): the kernels that

@@ -567,7 +567,7 @@ int adfb_block_set_bc(int blk, int nSub, const AdfbSubface* subfaces) {
         }
         b->subfaces.push_back(sf);
     }
-    // device-resident list of the subfaces for the two-launch BC path (k_bc_bulk / k_bc_frame)
+    // device-resident list of the subfaces for the SA wall terms (k_sa_bmt_all); null beyond ADFB_BC_MAXSUB subfaces
     b->dev.bcList = nullptr;
     BcList L;
     if (make_bc_list(b->d, b->subfaces, &L)) {
@@ -1085,7 +1085,7 @@ static int residual_body(int level, unsigned flags) {
         if (split && halo_exchange_impl(level, lStart, lEnd, 1, 1, ov, 1)) return 1;
         for (Block& b : g.blocks) {
             if (!b.alive || b.level != level) continue;
-            if (launch_bc_all(b.d, b.dev, b.subfaces, 1, g.prm.equations == ADFB_RANS && (flags & ADFB_RES_TURB), g.stream))
+            if (launch_bc_levels(b.d, b.dev, b.subfaces, 1, g.prm.equations == ADFB_RANS && (flags & ADFB_RES_TURB), 1, g.stream))
                 return fail("BC launch failed");
         }
         if (halo_exchange_impl(level, lStart, lEnd, 1, 1, ov, split ? 2 : 0)) return 1;
@@ -1094,7 +1094,7 @@ static int residual_body(int level, unsigned flags) {
             // present (blockette.F90:252-262): boundary halos next to fringe cells see the interpolated values
             for (Block& b : g.blocks) {
                 if (!b.alive || b.level != level) continue;
-                if (launch_bc_all(b.d, b.dev, b.subfaces, 1, g.prm.equations == ADFB_RANS && (flags & ADFB_RES_TURB), g.stream))
+                if (launch_bc_levels(b.d, b.dev, b.subfaces, 1, g.prm.equations == ADFB_RANS && (flags & ADFB_RES_TURB), 1, g.stream))
                     return fail("BC launch failed");
             }
         }
@@ -1512,7 +1512,7 @@ int adfb_apply_bcs(int level, int secondHalo, int withTurb) {
     if (!g.havePrm) return fail("adfb_apply_bcs: adfb_set_params has not been called");
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
-        if (launch_bc_all(b.d, b.dev, b.subfaces, secondHalo, withTurb && g.prm.equations == ADFB_RANS, g.stream)) return fail("BC launch failed");
+        if (launch_bc_levels(b.d, b.dev, b.subfaces, secondHalo, withTurb && g.prm.equations == ADFB_RANS, 1, g.stream)) return fail("BC launch failed");
     }
     return 0;
 }
@@ -1580,7 +1580,7 @@ static int adfb_rk_stage_body(int level, int rkStage) {
     if (split && halo_exchange_impl(level, 1, 5, 1, 1, overset_present(level), 1)) return 1;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
-        if (launch_bc_flow(b.d, b.dev, b.subfaces, above_ground(level) ? 0 : 1, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(b.d, b.dev, b.subfaces, above_ground(level) ? 0 : 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (halo_exchange_impl(level, 1, 5, 1, 1, overset_present(level), split ? 2 : 0)) return 1;
     CK(cudaGetLastError());
@@ -1604,7 +1604,7 @@ static int adfb_dadi_step_body(int level) {
         if (level > 1) prmL.cfl = g.prm.cflCoarse;
         if (launch_dadi(b.d, b.dev, prmL, g.stream)) return fail("DADI launch failed");
         if (launch_dadi_update(b.d, b.dev, prmL, g.stream, above_ground(level) ? 5 : 0)) return fail("DADI update launch failed");
-        if (launch_bc_flow(b.d, b.dev, b.subfaces, above_ground(level) ? 0 : 1, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(b.d, b.dev, b.subfaces, above_ground(level) ? 0 : 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (halo_exchange_impl(level, 1, 5, 1, 1, overset_present(level))) return 1;
     CK(cudaGetLastError());
@@ -2085,7 +2085,7 @@ static int adfb_mg_restrict_body(int fineLevel) {
         KT_BEGIN(K_MISC, g.stream);
         launch_pdl(k_mg_corner_rows, dim3(1), dim3(256), g.stream, c.d, c.dev);
         KT_END(K_MISC, g.stream);
-        if (launch_bc_flow(c.d, c.dev, c.subfaces, 0, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(c.d, c.dev, c.subfaces, 0, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (!any) return fail("adfb_mg_restrict: no blocks on level %d", cl);
     // whalo1(currentLevel, 1, nwf, T, T, T)
@@ -2143,7 +2143,7 @@ static int adfb_mg_prolong_body(int fineLevel) {
         launch_pdl(k_mg_prolong, gr, tb, g.stream, f.d, f.dev, c.d, c.dev, c.mg, f.nw);
         KT_END(K_MISC, g.stream);
         // applyAllBC(secondHalo): second halos on the ground level only
-        if (launch_bc_flow(f.d, f.dev, f.subfaces, above_ground(fineLevel) ? 0 : 1, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(f.d, f.dev, f.subfaces, above_ground(fineLevel) ? 0 : 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (halo_exchange_impl(fineLevel, 1, 5, 1, 1, overset_present(fineLevel))) return 1;
     CK(cudaGetLastError());
@@ -2214,16 +2214,16 @@ static int adfb_mg_prolong_solution_body(int fineLevel) {
             KT_END(K_MISC, g.stream);
         }
         const bool rans = g.prm.equations == ADFB_RANS;
-        if (rans && launch_bc_turb(f.d, f.dev, f.subfaces, 1, g.stream)) return fail("turbulence BC launch failed");
-        if (launch_bc_flow(f.d, f.dev, f.subfaces, 1, g.stream)) return fail("flow BC launch failed");
-        if (launch_bc_flow(f.d, f.dev, f.subfaces, 1, g.stream)) return fail("flow BC launch failed");
+        if (rans && launch_bc_levels(f.d, f.dev, f.subfaces, 1, 1, 0, g.stream)) return fail("turbulence BC launch failed");
+        if (launch_bc_levels(f.d, f.dev, f.subfaces, 1, 0, 1, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(f.d, f.dev, f.subfaces, 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     int nwAll = 5;
     for (Block& f : g.blocks) if (f.alive && f.level == fineLevel) nwAll = f.nw;
     if (halo_exchange_impl(fineLevel, 1, nwAll, 1, 1, overset_present(fineLevel))) return 1;
     for (Block& f : g.blocks) {
         if (!f.alive || f.level != fineLevel) continue;
-        if (launch_bc_flow(f.d, f.dev, f.subfaces, 1, g.stream)) return fail("flow BC launch failed");
+        if (launch_bc_levels(f.d, f.dev, f.subfaces, 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (halo_exchange_impl(fineLevel, 1, nwAll, 1, 1, overset_present(fineLevel))) return 1;
     CK(cudaGetLastError());

@@ -424,6 +424,6 @@ static int launch_sa_block(const Dims& d, const BlockDev& b, const AdfbParams& p
         launch_pdl(k_sa_update, g, tb, s, d, b);
         KT_END(K_SASOLVE, s);
     }
-    if (launch_bc_turb(d, b, subs, 1, s)) return 1;
+    if (launch_bc_levels(d, b, subs, 1, 1, 0, s)) return 1;
     return (int)cudaGetLastError();
 }

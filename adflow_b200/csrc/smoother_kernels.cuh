@@ -1,16 +1,16 @@
 // smoother_kernels.cuh -- boundary-condition, Runge-Kutta and residual-averaging kernels
 //
-//   k_bc_turb / k_bc_flow : applyAllTurbBCThisBlock (src/turbulence/turbBCRoutines.F90:49-236)
-//                           and applyAllBC_block (src/solver/BCRoutines.F90:57-222) for the BC
-//                           classes: symmetry, adiabatic / isothermal NS wall,
-//                           far field, extrapolation, Euler wall.  One launch per subface and phase, issued
-//                           in the reference's order (edge/corner halos depend on it).
+//   k_bc_level  : applyAllTurbBCThisBlock (src/turbulence/turbBCRoutines.F90:49-236) and applyAllBC_block
+//                 (src/solver/BCRoutines.F90:57-222) for the BC classes symmetry, polar symmetry, adiabatic /
+//                 isothermal NS wall, far field, sub- / supersonic in- and outflow, extrapolation and Euler wall.
+//                 launch_bc_levels issues the reference's ordered (subface, phase) items as levels of mutually
+//                 independent items, one launch per level, so the edge / corner halos keep the reference's order.
 //   k_rk_scale / k_rk_update : executeRkStage (src/solver/smoothers.F90:90-382)
-//   k_resavg_line            : residualAveraging (src/solver/residuals.F90:1785-2080)
+//   k_resavg_rfl / k_resavg_eps / k_resavg_sweep / k_resavg_lines : residualAveraging (src/solver/residuals.F90:1785-2080)
+//   k_wall_forces : wallIntegrationFace, forces and moments (src/solver/surfaceIntegrations.F90:406-881)
 #pragma once
 #include "adfb_common.cuh"
 #include <math.h>
-#include <cooperative_groups.h>
 
 struct FaceDev {
     long long off[4];  // plane 0 (2nd halo) .. 3 (2nd interior), setBCPointers utils.F90:881
@@ -326,197 +326,13 @@ __device__ __forceinline__ void bc_flow_cell(const Dims& d, const BlockDev& b, c
     }
 }
 
-// one launch per subface and phase (general path: more than ADFB_BC_MAXSUB subfaces on a block)
-__global__ void __launch_bounds__(128) k_bc_turb(Dims d, BlockDev b, FaceDev f, int secondHalo) {
-    // launched with programmatic stream serialization: the launch overlaps the tail of the previous
-    // kernel, the data dependency is honoured here
-    ADFB_PDL_SYNC();
-    const int ia = blockIdx.x * blockDim.x + threadIdx.x + f.icBeg;
-    const int jb = blockIdx.y * blockDim.y + threadIdx.y + f.jcBeg;
-    if (ia > f.icEnd || jb > f.jcEnd) return;
-    bc_turb_cell(d, b, f, ia, jb, secondHalo);
-}
-__global__ void __launch_bounds__(128) k_bc_flow(Dims d, BlockDev b, FaceDev f, int secondHalo, int phase) {
-    ADFB_PDL_SYNC();
-    const int ia = blockIdx.x * blockDim.x + threadIdx.x + f.icBeg;
-    const int jb = blockIdx.y * blockDim.y + threadIdx.y + f.jcBeg;
-    if (ia > f.icEnd || jb > f.jcEnd) return;
-    bc_flow_cell(d, b, f, ia, jb, secondHalo, phase);
-}
-
-// ---------------------------------------------------------------------------
-// All BCs of a block in TWO launches.  The order in which applyAllBC_block / applyAllTurbBCThisBlock visit the
-// subfaces only matters where subfaces touch common cells.  A face cell (a, b) reads the two owned cells and writes the
-// two halo cells of its own grid line, so it can only meet a subface of an adjacent face when one of its in-plane indices
-// lies within three cells of that face (indices 0..3 or l-1..l+1, see k_bc_sweep below).  So
-//   k_bc_bulk  : the cells with in-plane indices 4 .. l-2 of ALL subfaces at once (turbulence BC, then the flow BC incl.
-//                both symmetry phases): no other subface reads or writes their cells, any order is the reference's, and
-//   k_bc_frame : the rest of every subface (three layers along each block edge), one CTA walking the reference's ordered
-//                list of (subface, phase) items with a barrier between items.
-// (The whole owned range 2 .. l is NOT conflict-free: a frame cell of one subface reads the halo that an adjacent subface
-// later in the reference's order writes from its owned-range cells.)
-__device__ __forceinline__ void bc_bulk_box(const FaceDev& f, int la, int lb, int* a0, int* a1, int* b0, int* b1) {
-    *a0 = f.icBeg > 4 ? f.icBeg : 4; *a1 = f.icEnd < la - 2 ? f.icEnd : la - 2;
-    *b0 = f.jcBeg > 4 ? f.jcBeg : 4; *b1 = f.jcEnd < lb - 2 ? f.jcEnd : lb - 2;
-    if (*a1 < *a0 || *b1 < *b0) { *a0 = f.icBeg; *a1 = f.icEnd; *b0 = f.jcEnd + 1; *b1 = f.jcEnd; }   // no bulk: all rows are frame
-}
+// the subfaces of a block as a device-resident list (adfb_block_set_bc uploads it, k_sa_bmt_all reads it)
 #define ADFB_BC_MAXSUB 12
 struct BcList {
     int n;
     int la[ADFB_BC_MAXSUB], lb[ADFB_BC_MAXSUB];   // owned upper index of the two in-plane directions (il/jl/kl)
     FaceDev f[ADFB_BC_MAXSUB];
-    unsigned counters[2];   // k_bc_chain: tickets handed out, CTAs finished (zero between launches)
 };
-// the ordered (subface, kind) items of one BC sweep: kind 3 = turbulence BC, else the flow phase (1 / 2: symmetry first /
-// second halo, 0: everything else); begin[q] = first CTA ticket of item q
-#define ADFB_BC_MAXITEMS (4 * ADFB_BC_MAXSUB + 4)
-struct BcItems {
-    int n, total;
-    short sub[ADFB_BC_MAXITEMS], kind[ADFB_BC_MAXITEMS];
-    int begin[ADFB_BC_MAXITEMS + 1];
-};
-
-__device__ __forceinline__ void bc_all_cell(const Dims& d, const BlockDev& b, const FaceDev& f, int ia, int jb, int secondHalo,
-                                            int withTurb, int withFlow) {
-    if (withTurb) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-    if (!withFlow) return;
-    if (f.bcType == ADFB_BC_SYMM || f.bcType == ADFB_BC_SYMMPOLAR) {
-        bc_flow_cell(d, b, f, ia, jb, secondHalo, 1);
-        if (secondHalo) bc_flow_cell(d, b, f, ia, jb, secondHalo, 2);
-    } else {
-        bc_flow_cell(d, b, f, ia, jb, secondHalo, 0);
-    }
-}
-__global__ void __launch_bounds__(128) k_bc_bulk(Dims d, BlockDev b, const BcList* __restrict__ Lp, int secondHalo, int withTurb, int withFlow) {
-    ADFB_PDL_SYNC();
-    const BcList& L = *Lp;
-    const int s = blockIdx.z;
-    const FaceDev& f = L.f[s];
-    int a0, a1, b0, b1;
-    bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
-    const int ia = blockIdx.x * blockDim.x + threadIdx.x + a0;
-    const int jb = blockIdx.y * blockDim.y + threadIdx.y + b0;
-    if (ia > a1 || jb > b1) return;
-    bc_all_cell(d, b, f, ia, jb, secondHalo, withTurb, withFlow);
-}
-// the q-th frame cell of subface range [ic0..ic1] x [jc0..jc1] around the owned box [a0..a1] x [b0..b1]
-__device__ __forceinline__ bool frame_cell(int q, int ic0, int ic1, int jc0, int jc1, int a0, int a1, int b0, int b1, int* ia, int* jb) {
-    const int na = ic1 - ic0 + 1;
-    const int rowsLo = (b0 - jc0) > 0 ? (b0 - jc0) : 0, rowsHi = (jc1 - b1) > 0 ? (jc1 - b1) : 0;
-    int n = rowsLo * na;
-    if (q < n) { *ia = ic0 + q % na; *jb = jc0 + q / na; return true; }
-    q -= n;
-    n = rowsHi * na;
-    if (q < n) { *ia = ic0 + q % na; *jb = b1 + 1 + q / na; return true; }
-    q -= n;
-    const int colsLo = (a0 - ic0) > 0 ? (a0 - ic0) : 0, colsHi = (ic1 - a1) > 0 ? (ic1 - a1) : 0;
-    const int nbMid = (b1 >= b0) ? (b1 - b0 + 1) : 0, nc = colsLo + colsHi;
-    if (nc == 0 || q >= nc * nbMid) return false;
-    const int col = q % nc;
-    *jb = b0 + q / nc;
-    *ia = col < colsLo ? ic0 + col : a1 + 1 + (col - colsLo);
-    return true;
-}
-__global__ void __launch_bounds__(256) k_bc_frame(Dims d, BlockDev b, const BcList* __restrict__ Lp, int secondHalo, int withTurb, int withFlow) {
-    ADFB_PDL_SYNC();
-    const BcList& L = *Lp;
-    // ordered items: (subface, kind) with kind 3 = turbulence BC, else the flow phase
-    __shared__ short itemS[4 * ADFB_BC_MAXSUB + 4], itemK[4 * ADFB_BC_MAXSUB + 4];
-    __shared__ int nItems;
-    if (threadIdx.x == 0) {
-        int n = 0;
-        if (withTurb) for (int s = 0; s < L.n; s++) { itemS[n] = (short)s; itemK[n++] = 3; }
-        if (withFlow) {
-            for (int s = 0; s < L.n; s++) if (L.f[s].bcType == ADFB_BC_SYMM) { itemS[n] = (short)s; itemK[n++] = 1; }
-            if (secondHalo) for (int s = 0; s < L.n; s++) if (L.f[s].bcType == ADFB_BC_SYMM) { itemS[n] = (short)s; itemK[n++] = 2; }
-            for (int s = 0; s < L.n; s++) if (L.f[s].bcType == ADFB_BC_SYMMPOLAR) { itemS[n] = (short)s; itemK[n++] = 1; }
-            if (secondHalo) for (int s = 0; s < L.n; s++) if (L.f[s].bcType == ADFB_BC_SYMMPOLAR) { itemS[n] = (short)s; itemK[n++] = 2; }
-            const int order[8][2] = {{ADFB_BC_NSWALL_ADIABATIC, -1}, {ADFB_BC_NSWALL_ISOTHERMAL, -1}, {ADFB_BC_FARFIELD, -1},
-                                     {ADFB_BC_SUBSONIC_OUTFLOW, -1}, {ADFB_BC_SUBSONIC_INFLOW, -1}, {ADFB_BC_EXTRAP, ADFB_BC_SUPERSONIC_OUTFLOW},
-                                     {ADFB_BC_EULERWALL, -1}, {ADFB_BC_SUPERSONIC_INFLOW, -1}};
-            for (int g = 0; g < 8; g++)
-                for (int s = 0; s < L.n; s++)
-                    if (L.f[s].bcType == order[g][0] || L.f[s].bcType == order[g][1]) { itemS[n] = (short)s; itemK[n++] = 0; }
-        }
-        nItems = n;
-    }
-    __syncthreads();
-    for (int it = 0; it < nItems; it++) {
-        const int s = itemS[it], kind = itemK[it];
-        const FaceDev& f = L.f[s];
-        int a0, a1, b0, b1;
-        bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
-        for (int q = threadIdx.x;; q += blockDim.x) {
-            int ia, jb;
-            if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) break;
-            if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-            else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-        }
-        __syncthreads();
-    }
-}
-
-// The whole ordered BC sweep of a block in ONE launch.  The reference applies the subfaces one after the other
-// (applyAllTurbBCThisBlock, then applyAllBC_block in its BC-class order, BCRoutines.F90:81-216), and the edge / corner
-// halos depend on that order, so the items stay strictly ordered -- but the hand-over from one item to the next is a
-// device-side counter instead of a kernel boundary (a dependent launch inside a graph): a CTA draws a ticket,
-// which names its item and its 32 x 4 patch of the subface, waits until every CTA of all earlier items has finished
-// (tickets are handed out in start order, so everything a CTA waits for is already running: no deadlock whatever the
-// dispatch order), applies the BC, and publishes its completion.
-__device__ __forceinline__ unsigned bc_ld_acquire(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__global__ void __launch_bounds__(128) k_bc_chain(Dims d, BlockDev b, BcList* Lp, BcItems it, int secondHalo) {
-    ADFB_PDL_SYNC();
-    __shared__ int sTicket;
-    BcList& L = *Lp;
-    const bool t0 = threadIdx.x == 0 && threadIdx.y == 0;
-    if (t0) sTicket = (int)atomicAdd(&L.counters[0], 1u);
-    __syncthreads();
-    const int ticket = sTicket;
-    int q = 0;
-    while (q + 1 < it.n && ticket >= it.begin[q + 1]) q++;
-    const int local = ticket - it.begin[q];
-    const FaceDev& f = L.f[it.sub[q]];
-    const int kind = it.kind[q];
-    const int na = f.icEnd - f.icBeg + 1;
-    const int nbx = (na + 31) / 32;
-    const int ia = (local % nbx) * 32 + threadIdx.x + f.icBeg, jb = (local / nbx) * 4 + threadIdx.y + f.jcBeg;
-    if (t0) {
-        while (bc_ld_acquire(&L.counters[1]) < (unsigned)it.begin[q]) __nanosleep(40);
-    }
-    __syncthreads();
-    if (ia <= f.icEnd && jb <= f.jcEnd) {
-        if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-        else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-    }
-    __threadfence();
-    __syncthreads();
-    if (t0) {
-        const unsigned old = atomicAdd(&L.counters[1], 1u);
-        if ((int)old + 1 == it.total) {   // last CTA of the sweep: every ticket has been drawn, rearm the counters
-            L.counters[0] = 0u;
-            L.counters[1] = 0u;
-            __threadfence();
-        }
-    }
-}
-
-// one ordered frame item (subface s of the list, kind 3 = turbulence BC, else the flow phase): the frame cells only
-__global__ void __launch_bounds__(128) k_bc_frame_item(Dims d, BlockDev b, const BcList* __restrict__ Lp, int s, int kind, int secondHalo) {
-    ADFB_PDL_SYNC();
-    const BcList& L = *Lp;
-    const FaceDev& f = L.f[s];
-    int a0, a1, b0, b1;
-    bc_bulk_box(f, L.la[s], L.lb[s], &a0, &a1, &b0, &b1);
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    int ia, jb;
-    if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) return;
-    if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-    else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-}
 
 // One LEVEL of the ordered BC sweep.  Two items of the reference's ordered list (subface, kind) can only influence each other
 // when they touch common cells: subfaces on faces of different index directions (they share the edge / corner halos of
@@ -524,7 +340,7 @@ __global__ void __launch_bounds__(128) k_bc_frame_item(Dims d, BlockDev b, const
 // Subfaces on opposite faces, disjoint subfaces of one face and the two symmetry phases of one subface read and write
 // disjoint cells.  Items are given the level 1 + max(level of the earlier items they conflict with); the items of one level
 // run in one launch (blockIdx.z = item), the levels in the reference's order -- every conflicting pair keeps its order,
-// so the halos are the reference's bit for bit, in about half the launches.
+// so the halos are the reference's bit for bit, in about half as many launches as one per item.
 #define ADFB_BC_LEVEL_MAX 8
 struct BcLevel {   // passed by value: the face descriptors sit in the constant bank, no dependent global load before the state loads
     int n;
@@ -540,102 +356,6 @@ __global__ void __launch_bounds__(128) k_bc_level(Dims d, BlockDev b, const __gr
     if (ia > f.icEnd || jb > f.jcEnd || jb < f.bLo || jb > f.bHi) return;
     if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
     else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-}
-
-// The whole ordered BC sweep of a block in ONE launch, exact.  A face cell (a, b) of a subface reads the two owned cells
-// and writes the two halo cells of its own grid line; it can only meet cells of a subface of an ADJACENT face when one of its
-// in-plane indices lies within three cells of that face (indices 0..3 or l-1..l+1: the neighbour's halos 0, 1 and the owned
-// cells 2, 3 its BC reads -- and vice versa).  So
-//   bulk  = in-plane indices 4 .. l-2 in both directions: conflict-free with every other subface, any order;
-//   frame = the rest of the subface (three layers along each block edge): applied in the reference's order.
-// CTA 0 walks the LEVELS of the ordered item list (bc_items_conflict) over the frames with a barrier between levels --
-// a frame level is ~1000 cells, one pass of the CTA -- while the other CTAs apply turbulence + flow BCs to the bulk cells.
-struct BcSweep {
-    int nLevels, nItems;
-    short sub[ADFB_BC_MAXITEMS], kind[ADFB_BC_MAXITEMS];   // items sorted by level (stable)
-    short levelBegin[ADFB_BC_MAXITEMS + 1];
-    int bulkBegin[ADFB_BC_MAXSUB + 1];                      // first bulk CTA of every subface (32 x 16 patches)
-    int nSub, la[ADFB_BC_MAXSUB], lb[ADFB_BC_MAXSUB];       // by value (constant bank): no dependent global load before the state loads
-    FaceDev f[ADFB_BC_MAXSUB];
-};
-__global__ void __launch_bounds__(512) k_bc_sweep(Dims d, BlockDev b, const BcList* __restrict__ Lp, const __grid_constant__ BcSweep sw, int secondHalo, int withTurb,
-                                                  int withFlow) {
-    ADFB_PDL_SYNC();
-    (void)Lp;
-    if (blockIdx.x == 0) {
-        const int tid = threadIdx.y * 32 + threadIdx.x;
-        for (int l = 0; l < sw.nLevels; l++) {
-            for (int it = sw.levelBegin[l]; it < sw.levelBegin[l + 1]; it++) {
-                const int s = sw.sub[it], kind = sw.kind[it];
-                const FaceDev& f = sw.f[s];
-                int a0, a1, b0, b1;
-                bc_bulk_box(f, sw.la[s], sw.lb[s], &a0, &a1, &b0, &b1);
-                for (int q = tid;; q += 512) {
-                    int ia, jb;
-                    if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) break;
-                    if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-                    else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-                }
-            }
-            __syncthreads();
-        }
-        return;
-    }
-    const int cta = blockIdx.x - 1;
-    int s = 0;
-    while (s + 1 < sw.nSub && cta >= sw.bulkBegin[s + 1]) s++;
-    const FaceDev& f = sw.f[s];
-    int a0, a1, b0, b1;
-    bc_bulk_box(f, sw.la[s], sw.lb[s], &a0, &a1, &b0, &b1);
-    if (b1 < b0) return;
-    const int local = cta - sw.bulkBegin[s];
-    const int nbx = (a1 - a0 + 1 + 31) / 32;
-    const int ia = (local % nbx) * 32 + threadIdx.x + a0, jb = (local / nbx) * 16 + threadIdx.y + b0;
-    if (ia > a1 || jb > b1) return;
-    bc_all_cell(d, b, f, ia, jb, secondHalo, withTurb, withFlow);
-}
-
-// k_bc_sweep with the ordered frames walked by a CLUSTER of 8 CTAs (4096 threads: a whole frame level in one pass) that meet
-// at the hardware cluster barrier between levels (release / acquire at cluster scope: the halo cells written by one CTA are
-// visible to the next level's reads of another).  Cluster 0 walks the frames, the other clusters apply the bulk cells.
-#define ADFB_BC_CLUSTER 8
-__global__ void __cluster_dims__(ADFB_BC_CLUSTER, 1, 1) __launch_bounds__(512)
-k_bc_sweep_cluster(Dims d, BlockDev b, const BcList* __restrict__ Lp, const __grid_constant__ BcSweep sw, int secondHalo, int withTurb, int withFlow, int nBulk) {
-    ADFB_PDL_SYNC();
-    (void)Lp;
-    if (blockIdx.x < ADFB_BC_CLUSTER) {
-        cooperative_groups::cluster_group cl = cooperative_groups::this_cluster();
-        const int tid = (int)cl.block_rank() * 512 + threadIdx.y * 32 + threadIdx.x;
-        for (int l = 0; l < sw.nLevels; l++) {
-            for (int it = sw.levelBegin[l]; it < sw.levelBegin[l + 1]; it++) {
-                const int s = sw.sub[it], kind = sw.kind[it];
-                const FaceDev& f = sw.f[s];
-                int a0, a1, b0, b1;
-                bc_bulk_box(f, sw.la[s], sw.lb[s], &a0, &a1, &b0, &b1);
-                for (int q = tid;; q += 512 * ADFB_BC_CLUSTER) {
-                    int ia, jb;
-                    if (!frame_cell(q, f.icBeg, f.icEnd, f.jcBeg, f.jcEnd, a0, a1, b0, b1, &ia, &jb)) break;
-                    if (kind == 3) bc_turb_cell(d, b, f, ia, jb, secondHalo);
-                    else bc_flow_cell(d, b, f, ia, jb, secondHalo, kind);
-                }
-            }
-            if (l + 1 < sw.nLevels) cl.sync();
-        }
-        return;
-    }
-    const int cta = blockIdx.x - ADFB_BC_CLUSTER;
-    if (cta >= nBulk) return;
-    int s = 0;
-    while (s + 1 < sw.nSub && cta >= sw.bulkBegin[s + 1]) s++;
-    const FaceDev& f = sw.f[s];
-    int a0, a1, b0, b1;
-    bc_bulk_box(f, sw.la[s], sw.lb[s], &a0, &a1, &b0, &b1);
-    if (b1 < b0) return;
-    const int local = cta - sw.bulkBegin[s];
-    const int nbx = (a1 - a0 + 1 + 31) / 32;
-    const int ia = (local % nbx) * 32 + threadIdx.x + a0, jb = (local / nbx) * 16 + threadIdx.y + b0;
-    if (ia > a1 || jb > b1) return;
-    bc_all_cell(d, b, f, ia, jb, secondHalo, withTurb, withFlow);
 }
 
 // ---------------------------------------------------------------------------
@@ -968,19 +688,6 @@ __global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev
 
 }  // namespace
 
-// ADFB_BC_FUSED: 5 = the whole sweep in one launch, exact (k_bc_sweep: bulk cells by all CTAs, the ordered frames by CTA 0);
-// 6 = the same with the frames walked by a cluster of 8 CTAs (k_bc_sweep_cluster);
-// 4 = one launch per LEVEL of mutually independent items (k_bc_level); 0 = one launch per subface and phase over all of its cells, chained by programmatic dependent
-// launch (13 launches for the bench block); 3 = the whole ordered sweep in one launch, items ordered by a device-side
-// counter (k_bc_chain: parity-clean, but the ticket / fence / counter hand-over per item costs more than the launch chain);
-// 1 = one launch for the order-independent cells of all subfaces (k_bc_bulk), then the ordered frame items as small launches
-// (k_bc_frame_item, 14 launches); 2 = the same bulk launch + one CTA walking the frame items (k_bc_frame, slower).  All of them
-// are exact: tests/kernel_table.py runs the BC parity tests under each mode.
-static int bc_mode() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("ADFB_BC_FUSED"); v = e ? atoi(e) : 4; }
-    return v;
-}
 // the reference's ordered list of (subface, kind) items of one BC sweep (applyAllTurbBCThisBlock, then applyAllBC_block in its
 // BC-class order: BCRoutines.F90:81-216); kind 3 = turbulence BC, 1 / 2 = symmetry first / second halo, 0 = the other classes
 static std::vector<std::pair<int, int>> bc_ordered_items(const std::vector<AdfbSubface>& subs, int secondHalo, int withTurb, int withFlow) {
@@ -1021,7 +728,7 @@ static bool bc_items_conflict(const std::vector<AdfbSubface>& subs, std::pair<in
 static int launch_bc_levels(const Dims& d, const BlockDev& b, const std::vector<AdfbSubface>& subs, int secondHalo, int withTurb, int withFlow,
                             cudaStream_t s, int bLo = -(1 << 30), int bHi = 1 << 30, int kFaces = 3) {
     const std::vector<std::pair<int, int>> items = bc_ordered_items(subs, secondHalo, withTurb, withFlow);
-    if (items.empty()) return 0;
+    if (items.empty()) return (int)cudaGetLastError();   // still reports a pending launch error
     std::vector<int> level(items.size(), 1);
     int nLevels = 1;
     for (size_t q = 0; q < items.size(); q++) {
@@ -1059,131 +766,6 @@ static int launch_bc_levels(const Dims& d, const BlockDev& b, const std::vector<
     }
     return (int)cudaGetLastError();
 }
-// all BCs of a block: bulk launch + ordered frames; returns -1 when the general path must be used
-static int launch_bc_fused(const Dims& d, const BlockDev& b, const std::vector<AdfbSubface>& subs, int secondHalo, int withTurb, int withFlow,
-                           cudaStream_t s) {
-    if (!bc_mode() || subs.empty()) return -1;
-    if (bc_mode() != 4 && ((int)subs.size() > ADFB_BC_MAXSUB || !b.bcList)) return -1;
-    if (bc_mode() == 5 || bc_mode() == 6) {
-        const std::vector<std::pair<int, int>> items = bc_ordered_items(subs, secondHalo, withTurb, withFlow);
-        if (items.empty()) return 0;
-        if ((int)items.size() > ADFB_BC_MAXITEMS) return -1;
-        std::vector<int> level(items.size(), 1);
-        int nLevels = 1;
-        for (size_t q = 0; q < items.size(); q++) {
-            for (size_t r = 0; r < q; r++)
-                if (level[r] >= level[q] && bc_items_conflict(subs, items[r], items[q])) level[q] = level[r] + 1;
-            if (level[q] > nLevels) nLevels = level[q];
-        }
-        BcSweep sw;
-        memset(&sw, 0, sizeof sw);
-        sw.nLevels = nLevels;
-        for (int l = 1; l <= nLevels; l++) {
-            sw.levelBegin[l - 1] = (short)sw.nItems;
-            for (size_t q = 0; q < items.size(); q++)
-                if (level[q] == l) { sw.sub[sw.nItems] = (short)items[q].first; sw.kind[sw.nItems] = (short)items[q].second; sw.nItems++; }
-        }
-        sw.levelBegin[nLevels] = (short)sw.nItems;
-        int nBulk = 0;
-        for (size_t q = 0; q < subs.size(); q++) {
-            const AdfbSubface& sf = subs[q];
-            const int la = (sf.faceId == ADFB_IMIN || sf.faceId == ADFB_IMAX) ? d.jl : d.il;
-            const int lb = (sf.faceId == ADFB_KMIN || sf.faceId == ADFB_KMAX) ? d.jl : d.kl;
-            const int a0 = std::max(sf.icBeg, 4), a1 = std::min(sf.icEnd, la - 2), b0 = std::max(sf.jcBeg, 4), b1 = std::min(sf.jcEnd, lb - 2);
-            sw.bulkBegin[q] = nBulk;
-            sw.f[q] = make_face(d, sf); sw.la[q] = la; sw.lb[q] = lb;
-            if (a1 >= a0 && b1 >= b0) nBulk += ((a1 - a0 + 1 + 31) / 32) * ((b1 - b0 + 1 + 15) / 16);
-        }
-        sw.bulkBegin[subs.size()] = nBulk;
-        sw.nSub = (int)subs.size();
-        KT_BEGIN(K_BC, s);
-        if (bc_mode() == 6) {
-            const unsigned nCta = (unsigned)(ADFB_BC_CLUSTER + (nBulk + ADFB_BC_CLUSTER - 1) / ADFB_BC_CLUSTER * ADFB_BC_CLUSTER);
-            launch_pdl(k_bc_sweep_cluster, dim3(nCta), dim3(32, 16), s, d, b, (const BcList*)b.bcList, sw, secondHalo, withTurb, withFlow, nBulk);
-        } else {
-            launch_pdl(k_bc_sweep, dim3((unsigned)(1 + nBulk)), dim3(32, 16), s, d, b, (const BcList*)b.bcList, sw, secondHalo, withTurb, withFlow);
-        }
-        KT_END(K_BC, s);
-        return (int)cudaGetLastError();
-    }
-    if (bc_mode() == 4) return launch_bc_levels(d, b, subs, secondHalo, withTurb, withFlow, s);
-    if (bc_mode() == 3) {
-        BcItems it;
-        memset(&it, 0, sizeof it);
-        int tot = 0;
-        auto item = [&](int q, int kind) {
-            const AdfbSubface& sf = subs[q];
-            const int na = sf.icEnd - sf.icBeg + 1, nb = sf.jcEnd - sf.jcBeg + 1;
-            it.sub[it.n] = (short)q; it.kind[it.n] = (short)kind; it.begin[it.n] = tot;
-            tot += ((na + 31) / 32) * ((nb + 3) / 4);
-            it.n++;
-        };
-        const int n = (int)subs.size();
-        if (withTurb) for (int q = 0; q < n; q++) item(q, 3);
-        if (withFlow) {
-            for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMM) item(q, 1);
-            if (secondHalo) for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMM) item(q, 2);
-            for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMMPOLAR) item(q, 1);
-            if (secondHalo) for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMMPOLAR) item(q, 2);
-            const int order[8][2] = {{ADFB_BC_NSWALL_ADIABATIC, -1}, {ADFB_BC_NSWALL_ISOTHERMAL, -1}, {ADFB_BC_FARFIELD, -1},
-                                     {ADFB_BC_SUBSONIC_OUTFLOW, -1}, {ADFB_BC_SUBSONIC_INFLOW, -1}, {ADFB_BC_EXTRAP, ADFB_BC_SUPERSONIC_OUTFLOW},
-                                     {ADFB_BC_EULERWALL, -1}, {ADFB_BC_SUPERSONIC_INFLOW, -1}};
-            for (int gq = 0; gq < 8; gq++)
-                for (int q = 0; q < n; q++)
-                    if (subs[q].bcType == order[gq][0] || subs[q].bcType == order[gq][1]) item(q, 0);
-        }
-        if (it.n == 0) return 0;
-        it.begin[it.n] = tot;
-        it.total = tot;
-        KT_BEGIN(K_BC, s);
-        launch_pdl(k_bc_chain, dim3((unsigned)tot), dim3(32, 4), s, d, b, (BcList*)b.bcList, it, secondHalo);
-        KT_END(K_BC, s);
-        return (int)cudaGetLastError();
-    }
-    int ma = 1, mb = 1;
-    for (const AdfbSubface& sf : subs) {
-        const int la = (sf.faceId == ADFB_IMIN || sf.faceId == ADFB_IMAX) ? d.jl : d.il;
-        const int lb = (sf.faceId == ADFB_KMIN || sf.faceId == ADFB_KMAX) ? d.jl : d.kl;
-        if (la - 1 > ma) ma = la - 1;
-        if (lb - 1 > mb) mb = lb - 1;
-    }
-    dim3 tb(32, 4);
-    dim3 g((ma + 31) / 32, (mb + 3) / 4, (unsigned)subs.size());
-    const BcList* L = (const BcList*)b.bcList;
-    KT_BEGIN(K_BC, s);
-    launch_pdl(k_bc_bulk, g, tb, s, d, b, L, secondHalo, withTurb, withFlow);
-    KT_END(K_BC, s);
-    if (bc_mode() == 2) {
-        KT_BEGIN(K_BC, s);
-        launch_pdl(k_bc_frame, dim3(1), dim3(256), s, d, b, L, secondHalo, withTurb, withFlow);
-        KT_END(K_BC, s);
-        return (int)cudaGetLastError();
-    }
-    // ordered frame items, the reference's order (applyAllTurbBCThisBlock, then applyAllBC_block: BCRoutines.F90:81-216)
-    auto item = [&](int q, int kind) {
-        const AdfbSubface& sf = subs[q];
-        const int na = sf.icEnd - sf.icBeg + 1, nb = sf.jcEnd - sf.jcBeg + 1;
-        const int nFrame = na * nb;   // upper bound of the frame cells of one subface (frame_cell() rejects the rest)
-        KT_BEGIN(K_BC, s);
-        launch_pdl(k_bc_frame_item, dim3((nFrame + 127) / 128), dim3(128), s, d, b, L, q, kind, secondHalo);
-        KT_END(K_BC, s);
-    };
-    const int n = (int)subs.size();
-    if (withTurb) for (int q = 0; q < n; q++) item(q, 3);
-    if (withFlow) {
-        for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMM) item(q, 1);
-        if (secondHalo) for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMM) item(q, 2);
-        for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMMPOLAR) item(q, 1);
-        if (secondHalo) for (int q = 0; q < n; q++) if (subs[q].bcType == ADFB_BC_SYMMPOLAR) item(q, 2);
-        const int order[8][2] = {{ADFB_BC_NSWALL_ADIABATIC, -1}, {ADFB_BC_NSWALL_ISOTHERMAL, -1}, {ADFB_BC_FARFIELD, -1},
-                                 {ADFB_BC_SUBSONIC_OUTFLOW, -1}, {ADFB_BC_SUBSONIC_INFLOW, -1}, {ADFB_BC_EXTRAP, ADFB_BC_SUPERSONIC_OUTFLOW},
-                                 {ADFB_BC_EULERWALL, -1}, {ADFB_BC_SUPERSONIC_INFLOW, -1}};
-        for (int gq = 0; gq < 8; gq++)
-            for (int q = 0; q < n; q++)
-                if (subs[q].bcType == order[gq][0] || subs[q].bcType == order[gq][1]) item(q, 0);
-    }
-    return (int)cudaGetLastError();
-}
 // host image of the device-resident subface list of a block (uploaded by adfb_block_set_bc)
 static bool make_bc_list(const Dims& d, const std::vector<AdfbSubface>& subs, BcList* L) {
     if (subs.empty() || (int)subs.size() > ADFB_BC_MAXSUB) return false;
@@ -1196,63 +778,6 @@ static bool make_bc_list(const Dims& d, const std::vector<AdfbSubface>& subs, Bc
         L->lb[q] = (face == ADFB_KMIN || face == ADFB_KMAX) ? d.jl : d.kl;
     }
     return true;
-}
-
-static int launch_bc_turb(const Dims& d, const BlockDev& b, const std::vector<AdfbSubface>& subs, int secondHalo, cudaStream_t s) {
-    {
-        const int rc = launch_bc_fused(d, b, subs, secondHalo, 1, 0, s);
-        if (rc >= 0) return rc;
-    }
-    for (const AdfbSubface& sf : subs) {
-        FaceDev f = make_face(d, sf);
-        dim3 tb(32, 4);
-        dim3 g((f.icEnd - f.icBeg + 1 + 31) / 32, (f.jcEnd - f.jcBeg + 1 + 3) / 4);
-        KT_BEGIN(K_BC, s);
-        launch_pdl(k_bc_turb, g, tb, s, d, b, f, secondHalo);
-        KT_END(K_BC, s);
-    }
-    return (int)cudaGetLastError();
-}
-
-static void launch_bc_one(const Dims& d, const BlockDev& b, const AdfbSubface& sf, int secondHalo, int phase, cudaStream_t s) {
-    FaceDev f = make_face(d, sf);
-    dim3 tb(32, 4);
-    dim3 g((f.icEnd - f.icBeg + 1 + 31) / 32, (f.jcEnd - f.jcBeg + 1 + 3) / 4);
-    KT_BEGIN(K_BC, s);
-    launch_pdl(k_bc_flow, g, tb, s, d, b, f, secondHalo, phase);
-    KT_END(K_BC, s);
-}
-
-// applyAllBC_block order, src/solver/BCRoutines.F90:81-216
-static int launch_bc_flow(const Dims& d, const BlockDev& b, const std::vector<AdfbSubface>& subs, int secondHalo, cudaStream_t s) {
-    {
-        const int rc = launch_bc_fused(d, b, subs, secondHalo, 0, 1, s);
-        if (rc >= 0) return rc;
-    }
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SYMM) launch_bc_one(d, b, sf, secondHalo, 1, s);
-    if (secondHalo)
-        for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SYMM) launch_bc_one(d, b, sf, secondHalo, 2, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SYMMPOLAR) launch_bc_one(d, b, sf, secondHalo, 1, s);
-    if (secondHalo)
-        for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SYMMPOLAR) launch_bc_one(d, b, sf, secondHalo, 2, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_NSWALL_ADIABATIC) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_NSWALL_ISOTHERMAL) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_FARFIELD) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SUBSONIC_OUTFLOW) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SUBSONIC_INFLOW) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs)
-        if (sf.bcType == ADFB_BC_EXTRAP || sf.bcType == ADFB_BC_SUPERSONIC_OUTFLOW) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_EULERWALL) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    for (const AdfbSubface& sf : subs) if (sf.bcType == ADFB_BC_SUPERSONIC_INFLOW) launch_bc_one(d, b, sf, secondHalo, 0, s);
-    return (int)cudaGetLastError();
-}
-
-// turbulence BCs of all subfaces, then the flow BCs (blocketteRes :213-226, applyAllTurbBC + applyAllBC)
-static int launch_bc_all(const Dims& d, const BlockDev& b, const std::vector<AdfbSubface>& subs, int secondHalo, int withTurb, cudaStream_t s) {
-    const int rc = launch_bc_fused(d, b, subs, secondHalo, withTurb, 1, s);
-    if (rc >= 0) return rc;
-    if (withTurb && launch_bc_turb(d, b, subs, secondHalo, s)) return 1;
-    return launch_bc_flow(d, b, subs, secondHalo, s);
 }
 
 static int launch_residual_averaging(const Dims& d, const BlockDev& b, const AdfbParams& prm, cudaStream_t s) {

@@ -40,12 +40,6 @@ GENERAL = {"ADFB_FUSED": "0"}                           # general kernels instea
 GRAD_AOS = {"ADFB_GRAD_AOS": "1", "ADFB_FUSED": "0"}    # AoS nodal gradients (general kernels only)
 SPLIT_FACES = {"ADFB_SPLIT_FACES": "1"}                 # viscous face fluxes in two launches
 FUSED_SMOOTHER = {"ADFB_FUSED_SMOOTHER": "1"}           # tile kernel on the smoother path
-BC_PER_SUBFACE = {"ADFB_BC_FUSED": "0"}                 # one launch per subface and phase
-BC_BULK_ITEMS = {"ADFB_BC_FUSED": "1"}                  # bulk launch + one launch per ordered frame item
-BC_BULK_FRAME = {"ADFB_BC_FUSED": "2"}                  # bulk launch + one CTA walking the ordered frames
-BC_CHAIN = {"ADFB_BC_FUSED": "3"}                       # ordered sweep in one launch, device-side tickets
-BC_SWEEP = {"ADFB_BC_FUSED": "5"}                       # bulk + ordered frame levels in one launch
-BC_SWEEP_CLUSTER = {"ADFB_BC_FUSED": "6"}               # the same, frames walked by a CTA cluster
 DADI_SMEM = {"ADFB_DADI_SMEM": "1"}                     # DADI rows and solve in shared memory
 RESAVG_SWEEP = {"ADFB_RESAVG_SMEM": "0"}                # residual averaging without the shared-memory line solve
 SA_BMT_PER_SUBFACE = {"ADFB_SA_BMT_ONE": "0"}           # SA wall terms one launch per subface
@@ -59,15 +53,7 @@ TABLE = {
     "k_ankvec": reach(["tests/test_ank_gpu.py::test_device_gmres_on_the_matrix_free_operators[ANK]"]),
     "k_ankvec_turb": reach(["tests/test_ank_gpu.py::test_turbulence_ksp_pieces"]),
     "k_axpy_many": reach(["tests/test_ank_gpu.py::test_device_gmres_on_the_matrix_free_operators[ANK]"]),
-    "k_bc_bulk": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_BULK_FRAME),
-    "k_bc_chain": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_CHAIN),
-    "k_bc_flow": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_PER_SUBFACE),
-    "k_bc_frame": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_BULK_FRAME),
-    "k_bc_frame_item": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_BULK_ITEMS),
     "k_bc_level": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
-    "k_bc_sweep": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_SWEEP),
-    "k_bc_sweep_cluster": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_SWEEP_CLUSTER),
-    "k_bc_turb": reach(["tests/test_smoother_parity.py::test_bcs_match_oracle"], BC_PER_SUBFACE),
     "k_dadi_coef<0>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_coef<1>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_coef<2>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),

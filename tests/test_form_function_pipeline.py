@@ -10,7 +10,7 @@ import pytest
 
 from adflow_b200.solver import ADFLOW_B200
 
-from util import case, oracle_form_function, rel_l2
+from util import MANY, MIXED, case, oracle_form_function, rel_l2
 
 pytestmark = pytest.mark.gpu
 
@@ -31,9 +31,13 @@ def pinned(n):
     ((17, 13, 30), None, 8),                       # nz not a multiple of the chunk, odd NI (cp.async tiles instead of TMA)
     ((20, 12, 18), {"equationType": "Euler"}, 6),   # no SA row
     ((16, 12, 24), {"equationType": "laminar NS"}, 4),
+    # faces split into pieces, piece boundaries along k inside slabs (tests/util.py: split_faces)
+    pytest.param(((24, 16, 32), MIXED), None, 6, id="MIXED"),
+    pytest.param(((24, 16, 32), MANY), None, 6, id="MANY"),
 ])
 def test_pipelined_form_function(cuda_lib, shape, options, slabs):
-    prm, hb = case(*shape, options)
+    shape, split = shape if len(shape) == 2 else (shape, None)
+    prm, hb = case(*shape, options, split=split)
     U = state_vec(hb)
     U = U * (1.0 + 1e-3 * np.random.default_rng(3).standard_normal(U.size))
     r_orc = oracle_form_function(prm, hb, U)

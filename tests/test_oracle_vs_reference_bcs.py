@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from oracle import refblockette as rb
-from util import case
+from util import MANY, MIXED, case
 
 pytestmark = pytest.mark.skipif(not rb.available(), reason="oracle/_ref/libblockette_ref.so not built")
 
@@ -42,9 +42,12 @@ def test_default_faces(eq, second):
     {IMIN: FAR, IMAX: WALL, JMIN: SYMM, JMAX: FAR, KMIN: FAR, KMAX: SYMM},
     {IMIN: SYMM, IMAX: SYMM, JMIN: WALL, JMAX: FAR, KMIN: FAR, KMAX: WALL},
     {IMIN: FAR, IMAX: FAR, JMIN: FAR, JMAX: WALL, KMIN: SYMM, KMAX: FAR},
+    pytest.param(MIXED, id="MIXED"),   # faces split into pieces (tests/util.py: split_faces)
+    pytest.param(MANY, id="MANY"),
 ])
 def test_every_face_orientation(perm):
-    prm, hb = case(8, 7, 9, {"equationType": "RANS"}, physical_faces=perm)
+    kw = {"split": perm} if perm in (MIXED, MANY) else {"physical_faces": perm}
+    prm, hb = case(8, 7, 9, {"equationType": "RANS"}, **kw)
     _check(prm, hb, True)
 
 
@@ -99,6 +102,8 @@ def test_euler_wall(const_p):
     {IMIN: EXTRAP, IMAX: FAR, JMIN: SYMM, JMAX: ISOWALL, KMIN: ISOWALL, KMAX: EXTRAP},
     {IMIN: SUBIN, IMAX: SUBOUT, JMIN: SUPIN, JMAX: SUPOUT, KMIN: WALL, KMAX: FAR},
     {IMIN: 11, IMAX: FAR, JMIN: SYMM, JMAX: 11, KMIN: WALL, KMAX: 11},   # polar symmetry: bcTurbSymm
+    pytest.param(MIXED, id="MIXED"),
+    pytest.param(MANY, id="MANY"),
 ])
 @pytest.mark.parametrize("second", [True, False])
 def test_turbulence_bcs(perm, second):
@@ -106,7 +111,7 @@ def test_turbulence_bcs(perm, second):
     bcTurbWall / bcTurbSymm / bcTurbFarfield, bcEddyWall / bcEddyNoWall and turb2ndHalo"""
     from oracle.pyoracle import Oracle
 
-    kw = {} if perm is None else {"physical_faces": perm}
+    kw = {} if perm is None else {"split": perm} if perm in (MIXED, MANY) else {"physical_faces": perm}
     prm, hb = case(8, 7, 9, {"equationType": "RANS"}, **kw)
     hb.subfaces.sort(key=lambda s_: 0 if s_["bcType"] in (2, 6) else 1)  # reference: viscous subfaces first
     ho = hb.copy()

@@ -7,7 +7,7 @@ from adflow_b200 import synthetic as syn
 from adflow_b200.solver import ADFLOW_B200
 from oracle.pyoracle import Oracle
 
-from util import case, rel_l2, rel_max
+from util import MANY, case, rel_l2, rel_max
 
 
 def test_oracle_strong_relaxation_limit():
@@ -46,9 +46,11 @@ def test_oracle_sa_residual_row_equals_blockette_row():
     ({"turbulenceProduction": "vorticity", "useft2SA": False}, (8, 9, 10), 1),
     (None, (20, 17, 16), 2),      # lines >= 16 cells: partitioned Thomas kernels (8 lanes per line)
     (None, (33, 40, 18), 1),
+    pytest.param(None, ((14, 11, 9), MANY), 1, id="MANY"),   # 14 subfaces: the SA wall terms one launch per subface
 ])
 def test_sa_ddadi_matches_oracle(cuda_lib, options, shape, niter):
-    prm, hb0 = case(*shape, options)
+    shape, split = shape if len(shape) == 2 else (shape, None)
+    prm, hb0 = case(*shape, options, split=split)
     ho = hb0.copy()
     o = Oracle(ho, prm)
     o.apply_turb_bc(True); o.apply_flow_bc(True)

@@ -5,7 +5,7 @@ import pytest
 from adflow_b200.solver import ADFLOW_B200, RES_FLOW, RES_TURB
 from oracle.pyoracle import Oracle
 
-from util import case, rel_l2, rel_max
+from util import MANY, MIXED, case, rel_l2, rel_max
 
 pytestmark = pytest.mark.gpu
 
@@ -27,9 +27,13 @@ POLAR_FACES = {1: 11, 2: 3, 3: 1, 4: 11, 5: 2, 6: 11}    # polar symmetry on a m
                                            (None, ISO_EXTRAP_FACES),
                                            ({"viscWallTreatment": "linear pressure extrapolation"}, ISO_EXTRAP_FACES),
                                            (None, INOUT_FACES), ({"equationType": "Euler"}, INOUT_FACES),
-                                           (None, POLAR_FACES)])
+                                           (None, POLAR_FACES),
+                                           pytest.param(None, MIXED, id="MIXED-RANS"),   # faces split into pieces
+                                           pytest.param({"equationType": "Euler"}, MIXED, id="MIXED-Euler"),
+                                           pytest.param(None, MANY, id="MANY-RANS")])
 def test_bcs_match_oracle(cuda_lib, options, faces):
-    prm, hb = case(13, 11, 9, options, **({} if faces is None else {"physical_faces": faces}))
+    kw = {} if faces is None else {"split": faces} if faces in (MIXED, MANY) else {"physical_faces": faces}
+    prm, hb = case(13, 11, 9, options, **kw)
     ho = hb.copy()
     o = Oracle(ho, prm)
     o.apply_turb_bc(True)
