@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from oracle import refblockette as rb
-from util import case
+from util import MIXED, case
 
 pytestmark = pytest.mark.skipif(not rb.available(), reason="oracle/_ref/libblockette_ref.so not built")
 
@@ -19,12 +19,17 @@ SYMM, WALL, FAR, EULERWALL, EXTRAP, ISOWALL = 1, 2, 3, 4, 5, 6
     {IMIN: WALL, IMAX: FAR, JMIN: FAR, JMAX: SYMM, KMIN: FAR, KMAX: WALL},
     {IMIN: FAR, IMAX: ISOWALL, JMIN: WALL, JMAX: FAR, KMIN: SYMM, KMAX: FAR},
     {IMIN: FAR, IMAX: FAR, JMIN: SYMM, JMAX: WALL, KMIN: WALL, KMAX: FAR},
+    # walls split into pieces (tests/util.py: split_faces): two wall pieces on KMIN, one on IMIN, an isothermal one on JMAX
+    pytest.param(MIXED, id="MIXED"),
 ])
 def test_wall_forces_match_reference(perm):
     from oracle.pyoracle import Oracle
 
-    kw = {} if perm is None else {"physical_faces": perm}
-    prm, hb = case(10, 9, 8, {"equationType": "RANS"}, **kw)
+    if perm is MIXED:
+        prm, hb = case(12, 9, 10, {"equationType": "RANS"}, split=MIXED)
+    else:
+        kw = {} if perm is None else {"physical_faces": perm}
+        prm, hb = case(10, 9, 8, {"equationType": "RANS"}, **kw)
     hb.subfaces.sort(key=lambda s_: 0 if s_["bcType"] in (2, 6) else 1)
     o = Oracle(hb, prm)
     o.apply_turb_bc(True); o.apply_flow_bc(True)
