@@ -62,7 +62,6 @@ struct BlockDev {
     // eddy viscosity, first-order dissipation: the currentLevel > groundLevel branches of the reference)
     double *wr, *w1, *p1;
     int coarse;
-    const void* bcList;   // device-resident BcList (smoother_kernels.cuh) of the block's subfaces for k_sa_bmt_all, or null
 };
 
 // Matrix-free product fused into the residual (NKSolvers.F90:437-461 with setW :1331 and setRVec :1262): the kernels that
@@ -162,11 +161,8 @@ struct KTimer {
 static KTimer g_kt;
 
 // lanes per line for the partitioned Thomas kernels (tridiag_part.cuh): 8 lanes x <= 16 rows, 16 lanes x <= 16
-// rows, or 0 = one thread per line (short or very long lines).  ADFB_PART=0 forces the serial kernels.
+// rows, or 0 = one thread per line (short or very long lines).
 static inline int adfb_part_lanes(int nl) {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("ADFB_PART"); enabled = e ? atoi(e) : 1; }
-    if (!enabled) return 0;
     if (nl >= 16 && nl <= 128) return 8;
     if (nl > 128 && nl <= 256) return 16;
     return 0;

@@ -567,16 +567,6 @@ int adfb_block_set_bc(int blk, int nSub, const AdfbSubface* subfaces) {
         }
         b->subfaces.push_back(sf);
     }
-    // device-resident list of the subfaces for the SA wall terms (k_sa_bmt_all); null beyond ADFB_BC_MAXSUB subfaces
-    b->dev.bcList = nullptr;
-    BcList L;
-    if (make_bc_list(b->d, b->subfaces, &L)) {
-        void* q = nullptr;
-        CK(cudaMalloc(&q, sizeof(BcList)));
-        b->bcAllocs.push_back(q);
-        CK(cudaMemcpy(q, &L, sizeof(BcList), cudaMemcpyHostToDevice));
-        b->dev.bcList = q;
-    }
     return 0;
 }
 

@@ -5,13 +5,11 @@
 // tridiagonal systems (3 distinct coefficient sets: u+-0, u+c, u-c) with the Thomas
 // algorithm (tridiagsolve, :1750-1783), and wraps the sweeps in cell-local changes of
 // basis (T_eta^-1 :1277-1327, T_xi^-1 T_eta :1407-1448, T_zeta^-1 T_xi :1543-1583,
-// T_zeta :1679-1731).  Here ONE kernel per sweep does everything for its direction:
-// the thread that owns a line applies the incoming change of basis while it reads dw,
-// builds the tridiagonal coefficients on the fly from w, p, rlv, rev and the metrics
-// (no qq/cc/dual_dt scratch arrays), eliminates forward, substitutes backward, and (k
-// sweep) applies T_zeta and the -1/vol scaling while it writes the result.
-// j and k lines are walked with threads adjacent in i (coalesced); i lines are walked
-// one thread per line.
+// T_zeta :1679-1731).  Each sweep is k_dadi_coef (cell coefficients, incoming change of
+// basis), k_dadi_tri (tridiagonal rows) and a Thomas walk; after the k sweep k_dadi_post
+// applies T_zeta and the -1/vol scaling (layout of the work arrays above k_dadi_coef).
+// j and k lines are walked by k_dadi_thomas, one thread per (line, variable), threads
+// adjacent in i (coalesced); i lines by k_dadi_thomas_tile, one warp per 32 lines.
 //
 // Reference quirks kept: the spectral_* terms are multiplied by zero (:1269-1271) and
 // vanish; the k sweep's eps2 metric uses sj for the lower face (:1625-1627).
@@ -456,100 +454,6 @@ __global__ void __launch_bounds__(32 * ADFB_DT_WARPS) k_dadi_thomas_tile(Dims d,
     }
 }
 
-// The three coefficient sets and the five right-hand sides of LPC grid lines solved in shared memory: replaces
-// k_dadi_tri + k_dadi_thomas (tridiagonal rows residuals.F90:1374-1391, tridiagsolve :1750-1783).
-//   A  all threads copy the cell coefficients of k_dadi_coef (dP, dM of the three sets, viscTerm1/3, dual_dt) and
-//      the five transformed residuals of the lines into shared memory, consecutive threads along the direction that
-//      is contiguous in HBM
-//   B  one thread per (line, coefficient set), the three of a line in one warp: rows and forward elimination;
-//      1/(cc - bb dd), bb and dd overwrite the coefficient arrays in place (the triple reads cell i and i+1 before
-//      it writes cell i)
-//   C  one thread per (line, variable): forward substitution and back substitution in place
-//   D  coalesced copy back to dw
-// Same operations on the same operands as k_dadi_tri / k_dadi_thomas; the work arrays no longer pass through HBM.
-#define ADFB_DL_THREADS 768
-template <int LPC>
-__global__ void __launch_bounds__(ADFB_DL_THREADS) k_dadi_lines(Dims d, BlockDev b, long long sd, int n, long long s1, int n1, long long s2, int n2) {
-    ADFB_PDL_SYNC();
-    extern __shared__ double dl_sm[];
-    constexpr int LP = LPC + 1;
-    const size_t A1 = (size_t)n * LP;      // one array
-    double* S = dl_sm;                     // [9][n][LP]: 0..2 dP_t -> d0_t, 3..5 dM_t -> bb_t, 6 vt1 -> dd_0, 7 vt3 -> dd_1, 8 dt -> dd_2
-    double* F = dl_sm + 9 * A1;            // [5][n][LP]
-    const int tid = threadIdx.x, nT = blockDim.x;
-    const int q1lo = blockIdx.x * LPC + 2, q2 = blockIdx.y + 2;
-    const int nLines = min(LPC, n1 + 2 - q1lo);
-    const long long N = d.N;
-    const bool alongLine = sd == 1;
-    const int total = n * nLines;
-    for (int e = tid; e < total; e += nT) {
-        const int i = alongLine ? e % n : e / nLines, ln = alongLine ? e / n : e % nLines;
-        const long long c = (q1lo + ln) * s1 + q2 * s2 + (i + 2) * sd;
-#pragma unroll
-        for (int v = 0; v < 9; v++) S[v * A1 + i * LP + ln] = b.flux[v * N + c];
-#pragma unroll
-        for (int v = 0; v < 5; v++) F[v * A1 + i * LP + ln] = b.dw[v * N + c];
-    }
-    __syncthreads();
-    {   // B: 10 lines x 3 sets per warp (lanes 30, 31 idle)
-        const int warp = tid >> 5, lane = tid & 31;
-        const int ln = warp * 10 + lane / 3, t = lane % 3;
-        const bool act = lane < 30 && ln < nLines;   // warp-uniform trip count below: inactive lanes just skip the accesses
-        if (warp * 10 < nLines) {
-            double dPm = 0.0, vt1m = 0.0, ddp = 0.0;
-            for (int i = 0; i < n; i++) {
-                double d0 = 0.0, bb = 0.0, ddm = 0.0;
-                if (act) {
-                    const size_t o = (size_t)i * LP + ln;
-                    const double dP = S[t * A1 + o], dM = S[(3 + t) * A1 + o], vt1 = S[6 * A1 + o], vt3 = S[7 * A1 + o], dt = S[8 * A1 + o];
-                    const double cc = 1.0 + ((vt1 + vt3) + dP - dM) * dt;
-                    bb = (i > 0) ? (-vt1m - dPm) * dt : 0.0;
-                    const double ds = (i < n - 1) ? (-S[7 * A1 + o + LP] + S[(3 + t) * A1 + o + LP]) * dt : 0.0;
-                    d0 = (i == 0) ? 1.0 / cc : 1.0 / (cc - bb * ddp);
-                    ddm = ds * d0;
-                    dPm = dP; vt1m = vt1; ddp = ddm;
-                }
-                __syncwarp();
-                if (act) {
-                    const size_t o = (size_t)i * LP + ln;
-                    S[t * A1 + o] = d0; S[(3 + t) * A1 + o] = bb; S[(6 + t) * A1 + o] = ddm;
-                }
-            }
-        }
-    }
-    __syncthreads();
-    {   // C: one thread per (line, variable)
-        const int ln = tid % LPC, m = tid / LPC;
-        if (m < 5 && ln < nLines) {
-            const int t = m < 3 ? 0 : m - 2;   // coefficient set: (u), (u+c), (u-c)
-            double* f = F + m * A1 + ln;
-            const double* d0A = S + t * A1 + ln;
-            const double* bbA = S + (3 + t) * A1 + ln;
-            const double* ddA = S + (6 + t) * A1 + ln;
-            double ffp = 0.0;
-#pragma unroll 8
-            for (int i = 0; i < n; i++) {
-                const double v = (i == 0) ? f[(size_t)i * LP] * d0A[(size_t)i * LP] : (f[(size_t)i * LP] - bbA[(size_t)i * LP] * ffp) * d0A[(size_t)i * LP];
-                f[(size_t)i * LP] = v;
-                ffp = v;
-            }
-#pragma unroll 8
-            for (int i = n - 2; i >= 0; i--) {
-                const double v = f[(size_t)i * LP] - ddA[(size_t)i * LP] * ffp;
-                f[(size_t)i * LP] = v;
-                ffp = v;
-            }
-        }
-    }
-    __syncthreads();
-    for (int e = tid; e < total; e += nT) {
-        const int i = alongLine ? e % n : e / nLines, ln = alongLine ? e / n : e % nLines;
-        const long long c = (q1lo + ln) * s1 + q2 * s2 + (i + 2) * sd;
-#pragma unroll
-        for (int v = 0; v < 5; v++) b.dw[v * N + c] = F[v * A1 + i * LP + ln];
-    }
-}
-
 }  // namespace
 
 // computedwDADI including the -cfl*dtl*vol scaling of executeDADIStep (smoothers.F90:515-528)
@@ -561,42 +465,9 @@ static int launch_dadi(const Dims& d, const BlockDev& b, const AdfbParams& prm, 
     // (a partitioned, 8-lanes-per-line variant of this solve was measured slower here: with 5 systems per line the
     // serial walks already fill the machine and the partition method does 2.5x the arithmetic; it pays for the
     // single-system SA solve only, see sa_kernels.cuh)
-    // ADFB_DADI_SMEM=1: rows + solve in shared memory (k_dadi_lines; parity-clean, slower on C2 than k_dadi_tri + the
-    // thread-per-(line, variable) walks: 14 arrays per line leave 16 lines per CTA and two waves)
-    static int smemLines = -1;
-    if (smemLines < 0) { const char* e = getenv("ADFB_DADI_SMEM"); smemLines = e ? atoi(e) : 0; }
-    auto lines_lpc = [&](int nl) {
-        const size_t lim = 220 * 1024;
-        auto bytes = [&](int lpc) { return (size_t)14 * nl * (lpc + 1) * sizeof(double); };
-        return !smemLines ? 0 : bytes(32) <= lim ? 32 : bytes(16) <= lim ? 16 : bytes(8) <= lim ? 8 : bytes(4) <= lim ? 4 : 0;
-    };
-    // rows + solve of one sweep; returns false when the line does not fit into shared memory (general kernels then)
-    auto lines = [&](int sd, int nl, int s1, int n1, int s2, int n2) -> bool {
-        const int lpc = lines_lpc(nl);
-        if (!lpc || nl <= 1) return false;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((n1 + lpc - 1) / lpc, n2); cfg.blockDim = dim3(ADFB_DL_THREADS);
-        cfg.dynamicSmemBytes = (size_t)14 * nl * (lpc + 1) * sizeof(double); cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-#define ADFB_DL_LAUNCH(L)                                                                                                     \
-    do {                                                                                                                      \
-        static bool once = false;                                                                                             \
-        if (!once) { cudaFuncSetAttribute(k_dadi_lines<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024); once = true; } \
-        cudaLaunchKernelEx(&cfg, k_dadi_lines<L>, d, b, (long long)sd, nl, (long long)s1, n1, (long long)s2, n2);              \
-    } while (0)
-        if (lpc == 32) ADFB_DL_LAUNCH(32); else if (lpc == 16) ADFB_DL_LAUNCH(16); else if (lpc == 8) ADFB_DL_LAUNCH(8); else ADFB_DL_LAUNCH(4);
-#undef ADFB_DL_LAUNCH
-        return true;
-    };
-    // ADFB_DADI_TILE: 1 (default) = the tiled walk for the i sweep (lines along the contiguous index), 2 = for all three
-    // sweeps, 0 = per-thread walks everywhere
-    static int tileMode = -1;
-    if (tileMode < 0) { const char* e = getenv("ADFB_DADI_TILE"); tileMode = e ? atoi(e) : 1; }
+    // i lines (sd == 1) take the tiled walk: in the per-thread walk neighbouring threads own lines a whole row apart
     auto thomas = [&](int sd, int nl, int s1, int n1, int s2, int n2) {
-        if (tileMode == 2 || (tileMode == 1 && sd == 1)) {
+        if (sd == 1) {
             static bool once = false;
             const size_t smem = sizeof(DtSmem) * ADFB_DT_WARPS;
             if (!once) { cudaFuncSetAttribute(k_dadi_thomas_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); once = true; }
@@ -613,14 +484,8 @@ static int launch_dadi(const Dims& d, const BlockDev& b, const AdfbParams& prm, 
         }
         launch_pdl(k_dadi_thomas, dim3((n1 + 31) / 32, n2, 5), tb, s, d, b, sd, nl, s1, n1, s2, n2);
     };
-    // rows + solve of one direction: shared-memory kernel, else k_dadi_tri + k_dadi_thomas
+    // rows + solve of one direction
     auto solve = [&](int sd, int dirIdx, int nl, int s1, int n1, int s2, int n2) {
-        if (lines_lpc(nl) && nl > 1) {
-            KT_BEGIN(K_DADI, s);
-            lines(sd, nl, s1, n1, s2, n2);
-            KT_END(K_DADI, s);
-            return;
-        }
         KT_BEGIN(K_DADI, s);
         launch_pdl(k_dadi_tri, gc, tc, s, d, b, sd, dirIdx);
         KT_END(K_DADI, s);

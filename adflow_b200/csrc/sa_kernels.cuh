@@ -2,7 +2,8 @@
 // sa_block / saSolve, src/turbulence/sa.F90:16-86, 717-1267)
 //
 //   k_sa_bmt    : bcTurbTreatment (turbBCRoutines.F90:662-797) for the scalar SA variable: the
-//                 1x1 "matrix" bmt of every boundary face cell, stored at its first-halo cell
+//                 1x1 "matrix" bmt of every boundary face cell next to an owned cell, stored at
+//                 its first-halo cell
 //   k_sa_rhs    : block-path saSource (:89-344) + turbAdvection (turbUtils.F90:828-1553) +
 //                 saViscous (:346-676) incl. the implicit diagonal qq; saResScale (:678-714)
 //   k_sa_line   : one dd-ADI sweep: per grid line a scalar tridiagonal system (diffusion +
@@ -18,32 +19,11 @@
 
 namespace {
 
-__global__ void __launch_bounds__(128) k_sa_bmt(Dims d, BlockDev b, FaceDev f) {
+// The subfaces of the list in one launch (blockIdx.z = subface).  The values are read at the first-halo cells next to OWNED
+// cells only (k_sa_rhs, k_sa_coef), so each subface is clipped to its owned in-plane range: no cell is written by two
+// subfaces and the launch order of the reference's loop does not matter.
+__global__ void __launch_bounds__(128) k_sa_bmt(Dims d, BlockDev b, const __grid_constant__ BcList L) {
     ADFB_PDL_SYNC();
-    const int ia = blockIdx.x * blockDim.x + threadIdx.x + f.icBeg;
-    const int jb = blockIdx.y * blockDim.y + threadIdx.y + f.jcBeg;
-    if (ia > f.icEnd || jb > f.jcEnd) return;
-    const long long N = d.N;
-    const long long c1 = f.off[1] + ia * f.sa + jb * f.sb;
-    const long long na = f.icEnd - f.icBeg + 1, nb = f.jcEnd - f.jcBeg + 1;
-    const long long o = (ia - f.icBeg) + na * (jb - f.jcBeg);
-    double bmt = -1.0;
-    if (f.bcType == ADFB_BC_NSWALL_ADIABATIC || f.bcType == ADFB_BC_NSWALL_ISOTHERMAL || f.bcType == ADFB_BC_SUBSONIC_INFLOW ||
-        f.bcType == ADFB_BC_SUPERSONIC_INFLOW) bmt = 1.0;   // bcTurbWall / bcTurbInflow
-    else if (f.bcType == ADFB_BC_FARFIELD) {
-        const double dot = f.norm[o] * c_prm.wInf[1] + f.norm[o + na * nb] * c_prm.wInf[2] + f.norm[o + 2 * na * nb] * c_prm.wInf[3] -
-                           (f.rface ? f.rface[o] : 0.0);
-        bmt = dot > 0.0 ? -1.0 : 0.0;
-    }
-    b.scratch[2 * N + c1] = bmt;
-}
-
-// the same for all subfaces of the device-resident list in one launch (blockIdx.z = subface).  The values are read at the
-// first-halo cells next to OWNED cells only (k_sa_rhs, k_sa_coef), so each subface is clipped to its owned in-plane range:
-// no cell is written by two subfaces and the launch order of the reference's loop does not matter.
-__global__ void __launch_bounds__(128) k_sa_bmt_all(Dims d, BlockDev b, const BcList* __restrict__ Lp) {
-    ADFB_PDL_SYNC();
-    const BcList& L = *Lp;
     const int q = blockIdx.z;
     const FaceDev& f = L.f[q];
     const int a0 = f.icBeg > 2 ? f.icBeg : 2, a1 = f.icEnd < L.la[q] ? f.icEnd : L.la[q];
@@ -57,7 +37,7 @@ __global__ void __launch_bounds__(128) k_sa_bmt_all(Dims d, BlockDev b, const Bc
     const long long o = (ia - f.icBeg) + na * (jb - f.jcBeg);
     double bmt = -1.0;
     if (f.bcType == ADFB_BC_NSWALL_ADIABATIC || f.bcType == ADFB_BC_NSWALL_ISOTHERMAL || f.bcType == ADFB_BC_SUBSONIC_INFLOW ||
-        f.bcType == ADFB_BC_SUPERSONIC_INFLOW) bmt = 1.0;
+        f.bcType == ADFB_BC_SUPERSONIC_INFLOW) bmt = 1.0;   // bcTurbWall / bcTurbInflow
     else if (f.bcType == ADFB_BC_FARFIELD) {
         const double dot = f.norm[o] * c_prm.wInf[1] + f.norm[o + na * nb] * c_prm.wInf[2] + f.norm[o + 2 * na * nb] * c_prm.wInf[3] -
                            (f.rface ? f.rface[o] : 0.0);
@@ -374,23 +354,12 @@ __global__ void __launch_bounds__(256) k_sa_update(Dims d, BlockDev b) {
 static int launch_sa_block(const Dims& d, const BlockDev& b, const AdfbParams& prm, const std::vector<AdfbSubface>& subs, cudaStream_t s) {
     const int sJ = (int)d.sJ, sK = (int)d.sK;
     cudaMemsetAsync(b.scratch + 2 * d.N, 0, sizeof(double) * d.N, s);
-    static int bmtOne = -1;
-    if (bmtOne < 0) { const char* e = getenv("ADFB_SA_BMT_ONE"); bmtOne = e ? atoi(e) : 1; }
-    const bool oneLaunch = bmtOne && b.bcList && !subs.empty() && (int)subs.size() <= ADFB_BC_MAXSUB;
-    if (oneLaunch) {
+    for (size_t q0 = 0; q0 < subs.size(); q0 += ADFB_BC_MAXSUB) {
+        const BcList L = make_bc_list(d, subs, q0);
         int ma = 1, mb = 1;
-        for (const AdfbSubface& sf : subs) { ma = std::max(ma, sf.icEnd - sf.icBeg + 1); mb = std::max(mb, sf.jcEnd - sf.jcBeg + 1); }
+        for (int q = 0; q < L.n; q++) { ma = std::max(ma, L.f[q].icEnd - L.f[q].icBeg + 1); mb = std::max(mb, L.f[q].jcEnd - L.f[q].jcBeg + 1); }
         KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_bmt_all, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)subs.size()), dim3(32, 4), s, d, b, (const BcList*)b.bcList);
-        KT_END(K_SASOLVE, s);
-    }
-    for (const AdfbSubface& sf : subs) {
-        if (oneLaunch) break;
-        FaceDev f = make_face(d, sf);
-        dim3 tb(32, 4);
-        dim3 g((f.icEnd - f.icBeg + 1 + 31) / 32, (f.jcEnd - f.jcBeg + 1 + 3) / 4);
-        KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_bmt, g, tb, s, d, b, f);
+        launch_pdl(k_sa_bmt, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)L.n), dim3(32, 4), s, d, b, L);
         KT_END(K_SASOLVE, s);
     }
     const double factor = 1.0 + (1.0 - prm.alfaTurb) / prm.alfaTurb;

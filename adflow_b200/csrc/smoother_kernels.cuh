@@ -326,7 +326,8 @@ __device__ __forceinline__ void bc_flow_cell(const Dims& d, const BlockDev& b, c
     }
 }
 
-// the subfaces of a block as a device-resident list (adfb_block_set_bc uploads it, k_sa_bmt_all reads it)
+// up to ADFB_BC_MAXSUB subfaces of a block, passed by value to one launch of the SA wall terms (k_sa_bmt); blocks with more
+// subfaces take one launch per ADFB_BC_MAXSUB of them
 #define ADFB_BC_MAXSUB 12
 struct BcList {
     int n;
@@ -766,18 +767,18 @@ static int launch_bc_levels(const Dims& d, const BlockDev& b, const std::vector<
     }
     return (int)cudaGetLastError();
 }
-// host image of the device-resident subface list of a block (uploaded by adfb_block_set_bc)
-static bool make_bc_list(const Dims& d, const std::vector<AdfbSubface>& subs, BcList* L) {
-    if (subs.empty() || (int)subs.size() > ADFB_BC_MAXSUB) return false;
-    memset(L, 0, sizeof(BcList));
-    L->n = (int)subs.size();
-    for (int q = 0; q < L->n; q++) {
-        L->f[q] = make_face(d, subs[q]);
-        const int face = subs[q].faceId;
-        L->la[q] = (face == ADFB_IMIN || face == ADFB_IMAX) ? d.jl : d.il;
-        L->lb[q] = (face == ADFB_KMIN || face == ADFB_KMAX) ? d.jl : d.kl;
+// the subfaces subs[q0], subs[q0 + 1], ... of a block, at most ADFB_BC_MAXSUB of them
+static BcList make_bc_list(const Dims& d, const std::vector<AdfbSubface>& subs, size_t q0) {
+    BcList L;
+    memset(&L, 0, sizeof(BcList));
+    L.n = (int)std::min(subs.size() - q0, (size_t)ADFB_BC_MAXSUB);
+    for (int q = 0; q < L.n; q++) {
+        L.f[q] = make_face(d, subs[q0 + q]);
+        const int face = subs[q0 + q].faceId;
+        L.la[q] = (face == ADFB_IMIN || face == ADFB_IMAX) ? d.jl : d.il;
+        L.lb[q] = (face == ADFB_KMIN || face == ADFB_KMAX) ? d.jl : d.kl;
     }
-    return true;
+    return L;
 }
 
 static int launch_residual_averaging(const Dims& d, const BlockDev& b, const AdfbParams& prm, cudaStream_t s) {
@@ -793,14 +794,12 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
         KT_END(K_RK, s);
     }
     dim3 tb(32, 2);
-    static int smemLines = -1;   // ADFB_RESAVG_SMEM=0: the thread-per-(line, variable) walk through global memory
-    if (smemLines < 0) { const char* e = getenv("ADFB_RESAVG_SMEM"); smemLines = e ? atoi(e) : 1; }
     auto run = [&](int dir, long long sd, int n, long long s1, int n1, long long s2, int n2) {
         if (n <= 1) return;
         KT_BEGIN(K_RK, s);
         const size_t lim = 220 * 1024;
         int LP = 0; size_t smem = 0;
-        const int lpc = !smemLines ? 0 : lines_per_cta((long long)n1 * n2, n, 8, ADFB_RA_THREADS / 5, lim, &LP, &smem);
+        const int lpc = lines_per_cta((long long)n1 * n2, n, 8, ADFB_RA_THREADS / 5, lim, &LP, &smem);
         if (lpc) {
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((unsigned)(((long long)n1 * n2 + lpc - 1) / lpc)); cfg.blockDim = dim3(ADFB_RA_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
@@ -811,7 +810,7 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
             static bool once = false;
             if (!once) { cudaFuncSetAttribute(k_resavg_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lim); once = true; }
             cudaLaunchKernelEx(&cfg, k_resavg_lines, d, b, dir, sd, n, s1, n1, s2, n2, lpc, LP);
-        } else {
+        } else {   // not even one line fits into shared memory (n >= 3520 cells)
             launch_pdl(k_resavg_sweep, dim3((n1 + 31) / 32, (n2 + 1) / 2, 5), tb, s, d, b, dir, sd, n, s1, n1, s2, n2);
         }
         KT_END(K_RK, s);

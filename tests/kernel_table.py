@@ -40,9 +40,6 @@ GENERAL = {"ADFB_FUSED": "0"}                           # general kernels instea
 GRAD_AOS = {"ADFB_GRAD_AOS": "1", "ADFB_FUSED": "0"}    # AoS nodal gradients (general kernels only)
 SPLIT_FACES = {"ADFB_SPLIT_FACES": "1"}                 # viscous face fluxes in two launches
 FUSED_SMOOTHER = {"ADFB_FUSED_SMOOTHER": "1"}           # tile kernel on the smoother path
-DADI_SMEM = {"ADFB_DADI_SMEM": "1"}                     # DADI rows and solve in shared memory
-RESAVG_SWEEP = {"ADFB_RESAVG_SMEM": "0"}                # residual averaging without the shared-memory line solve
-SA_BMT_PER_SUBFACE = {"ADFB_SA_BMT_ONE": "0"}           # SA wall terms one launch per subface
 
 TABLE = {
     "k_ank_phys": reach(["tests/test_ank_gpu.py::test_ank_physicality_check[True]"]),
@@ -57,10 +54,6 @@ TABLE = {
     "k_dadi_coef<0>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_coef<1>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_coef<2>": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
-    "k_dadi_lines<16>": reach(["tests/test_dadi.py::test_dadi_step_matches_oracle"], DADI_SMEM),
-    "k_dadi_lines<32>": reach(["tests/test_dadi.py::test_dadi_step_matches_oracle"], DADI_SMEM),
-    "k_dadi_lines<4>": reach(["tests/test_dadi.py::test_dadi_step_matches_oracle"], DADI_SMEM),
-    "k_dadi_lines<8>": reach(["tests/test_dadi.py::test_dadi_step_matches_oracle"], DADI_SMEM),
     "k_dadi_post": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_thomas": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_dadi_thomas_tile": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
@@ -147,12 +140,11 @@ TABLE = {
     "k_resavg_eps": reach(["tests/test_mg_gpu.py::test_multigrid_accelerates_convergence_like_the_oracle"]),
     "k_resavg_lines": reach(["tests/test_mg_gpu.py::test_multigrid_accelerates_convergence_like_the_oracle"]),
     "k_resavg_rfl": reach(["tests/test_mg_gpu.py::test_multigrid_accelerates_convergence_like_the_oracle"]),
-    "k_resavg_sweep": reach(["tests/test_smoother_parity.py::test_residual_averaging_matches_oracle"], RESAVG_SWEEP),
+    "k_resavg_sweep": reach(["tests/test_smoother_parity.py::test_residual_averaging_matches_oracle[shape3]"]),
     "k_rk_scale": reach(["tests/test_mg_gpu.py::test_multigrid_accelerates_convergence_like_the_oracle"]),
     "k_rk_update": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_sa": reach(["tests/test_ank_gpu.py::test_device_gmres_on_the_matrix_free_operators[ANK]"]),
-    "k_sa_bmt": reach(["tests/test_sa_solve.py::test_sa_ddadi_matches_oracle"], SA_BMT_PER_SUBFACE),
-    "k_sa_bmt_all": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
+    "k_sa_bmt": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother", "tests/test_sa_solve.py::test_sa_ddadi_matches_oracle"]),
     "k_sa_coef": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_sa_rhs": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),
     "k_sa_thomas": reach(["tests/test_mg_gpu.py::test_mg_cycle_with_dadi_smoother"]),

@@ -52,14 +52,13 @@ def test_oracle_dadi_smoother_reduces_residual():
     ({"equationType": "laminar NS"}, (9, 12, 8)),
     ({"resAveraging": "always", "CFL": 5.0}, (10, 9, 8)),
     (None, (1, 7, 6)),
-    (None, (20, 17, 16)),         # lines >= 16 cells: partitioned Thomas kernels (8 lanes per line)
+    (None, (20, 17, 16)),         # lines >= 16 cells: several 8-cell chunks of the Thomas walks
     ({"resAveraging": "always", "CFL": 5.0}, (33, 18, 40)),
     ({"equationType": "Euler"}, (16, 35, 9)),   # mixed: i, j partitioned, k serial
     ({"discretization": "central plus matrix dissipation", "equationType": "Euler"}, (12, 9, 10)),
     ({"discretization": "upwind", "equationType": "laminar NS"}, (12, 9, 10)),
     ({"discretization": "upwind"}, (12, 9, 10)),
-    # line lengths for each lines-per-CTA of the shared-memory solve (ADFB_DADI_SMEM=1, 14 arrays of nl (L + 1) doubles
-    # in 220 KiB): L = 32 up to 60 cells, 16 up to 118, 8 up to 223, 4 up to 402
+    # long i and j lines: the tiled i walk over many 8-cell chunks, in groups of 32 lines, most with a shorter last group
     (None, (60, 61, 4)),
     (None, (118, 119, 3)),
     (None, (223, 224, 2)),

@@ -2,7 +2,7 @@
 
 The tests of one environment (tests/kernel_table.py) run in one subprocess under the kernel_trace plugin, with
 ADFB_NO_GRAPH=1 so that each launch is reported by itself; the run must pass, and each kernel of the group must appear in
-the trace of one of its tests.  The switches that select a kernel (ADFB_DADI_SMEM, ADFB_SA_BMT_ONE, ...) stay exercised
+the trace of one of its tests.  The switches that select a kernel (ADFB_FUSED, ADFB_SPLIT_FACES, ...) stay exercised
 this way, and a change of the dispatch that leaves a kernel unreachable from its tests fails here."""
 import json
 import os

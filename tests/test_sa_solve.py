@@ -46,7 +46,7 @@ def test_oracle_sa_residual_row_equals_blockette_row():
     ({"turbulenceProduction": "vorticity", "useft2SA": False}, (8, 9, 10), 1),
     (None, (20, 17, 16), 2),      # lines >= 16 cells: partitioned Thomas kernels (8 lanes per line)
     (None, (33, 40, 18), 1),
-    pytest.param(None, ((14, 11, 9), MANY), 1, id="MANY"),   # 14 subfaces: the SA wall terms one launch per subface
+    pytest.param(None, ((14, 11, 9), MANY), 1, id="MANY"),   # 14 subfaces: the SA wall terms in two launches
 ])
 def test_sa_ddadi_matches_oracle(cuda_lib, options, shape, niter):
     shape, split = shape if len(shape) == 2 else (shape, None)

@@ -122,7 +122,9 @@ def test_rk_cycle_matches_oracle(cuda_lib, options):
         box_close(rlv[c1], ho.rlv[c1], 1e-11, "rlv")
 
 
-@pytest.mark.parametrize("shape", [(18, 7, 9), (20, 17, 16), (36, 19, 41)])
+# (3600, 4, 3): an i line too long for shared memory (8 arrays of n doubles over 220 KiB from n = 3520) takes k_resavg_sweep,
+# its j and k lines k_resavg_lines
+@pytest.mark.parametrize("shape", [(18, 7, 9), (20, 17, 16), (36, 19, 41), (3600, 4, 3)])
 def test_residual_averaging_matches_oracle(cuda_lib, shape):
     prm, hb = case(*shape, {"CFL": 6.0, "resAveraging": "always", "nRKStages": 1})
     # one RK stage with averaging: compare dw after the stage (scaled + smoothed)

@@ -61,8 +61,8 @@ _SYMM, _WALL, _FAR, _EXTRAP, _ISOWALL, _SUBOUT, _SUBIN = 1, 2, 3, 5, 6, 7, 8
 MIXED = {syn.IMIN: (1, [_FAR, _WALL], [2]), syn.IMAX: (1, [_SUBIN, _SUBOUT], [7]),
          syn.JMIN: (1, [_SYMM, _FAR], [4]), syn.JMAX: (1, [_FAR, _ISOWALL, _FAR], [3, 8]),
          syn.KMIN: (0, [_WALL, _WALL, _FAR], [4, 7]), syn.KMAX: (1, [_EXTRAP, _FAR], [5])}
-# MANY: five far-field pieces along k on both i faces, 14 subfaces in all: more than the device list of a block holds
-# (ADFB_BC_MAXSUB), and ten independent items in one level of the BC sweep, more than one launch carries
+# MANY: five far-field pieces along k on both i faces, 14 subfaces in all: more than one launch of the SA wall terms
+# carries (ADFB_BC_MAXSUB), and ten independent items in one level of the BC sweep, more than one launch carries
 # (ADFB_BC_LEVEL_MAX).
 # In both, a level of the sweep holds pieces of different lengths, the longest not first.
 MANY = {syn.IMIN: (1, [_FAR] * 5, [2, 3, 4, 6]), syn.IMAX: (1, [_FAR] * 5, [2, 3, 4, 6])}
