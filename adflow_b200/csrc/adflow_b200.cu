@@ -119,6 +119,14 @@ Context g;
 // currentLevel > groundLevel: the coarse-level branches of the smoother path (dw = wr start, first-order dissipation, first
 // halos only, frozen eddy viscosity, constant-pressure walls); levels <= groundLevel run the fine-grid routines.
 static inline bool above_ground(int level) { return level > g.groundLevel; }
+// The discretisation of a residual on `level`.  The blockette path (blocketteRes: adfb_residual, the form function, the
+// matrix-free products, ANK) selects spaceDiscr on every level (blockette.F90:637-653); the block path of the smoothers and
+// of multigrid (residual_block) selects spaceDiscrCoarse unless currentLevel == 1 (residuals.F90:71-75).  So a coarse ground
+// level of the full-multigrid start-up runs its first smoothing step on a residual of the fine discretisation (solveState's
+// computeResidualNK, solvers.F90:1014-1018) and every later one on the fine-grid routines of the coarse discretisation.
+static inline int residual_discr(int level, bool blockette) {
+    return (blockette || level == 1) ? g.prm.spaceDiscr : g.prm.spaceDiscrCoarse;
+}
 
 int fail(const char* fmt, ...) {
     char buf[1024];
@@ -408,6 +416,8 @@ int adfb_set_params(const AdfbParams* prm) {
     if (prm->equations < ADFB_EULER || prm->equations > ADFB_RANS) return fail("adfb_set_params: bad equations %d", prm->equations);
     if (prm->spaceDiscr != ADFB_DISS_SCALAR && prm->spaceDiscr != ADFB_DISS_MATRIX && prm->spaceDiscr != ADFB_UPWIND)
         return fail("adfb_set_params: unknown spaceDiscr %d", prm->spaceDiscr);
+    if (prm->spaceDiscrCoarse != ADFB_DISS_SCALAR && prm->spaceDiscrCoarse != ADFB_DISS_MATRIX && prm->spaceDiscrCoarse != ADFB_UPWIND)
+        return fail("adfb_set_params: unknown spaceDiscrCoarse %d", prm->spaceDiscrCoarse);
     if (prm->useRotationSA && prm->turbProd == ADFB_PROD_VORTICITY)
         return fail("adfb_set_params: useRotationSA with vorticity production reads an unset strainMag2 in the "
                     "reference (src/turbulence/sa.F90:273); unsupported");
@@ -1059,7 +1069,7 @@ static int residual_body(int level, unsigned flags) {
             CK(cudaStreamWaitEvent(s2, eFork, 0));
             for (Block& b : g.blocks) {
                 if (!b.alive || b.level != level) continue;
-                if (launch_residual_core(b.d, b.dev, g.prm, flags, 1.0, 0, 1, s2, 0, RC_PREP_OWNED | RC_SA_INNER))
+                if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, true), flags, 1.0, 0, 1, s2, 0, RC_PREP_OWNED | RC_SA_INNER))
                     return fail("residual kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
             }
             CK(cudaEventRecord(eJoin, s2));
@@ -1095,7 +1105,7 @@ static int residual_body(int level, unsigned flags) {
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         const MffdEpi mf = {g.mffdFuse ? g.dMffd : nullptr, cell0};
-        if (launch_residual_core(b.d, b.dev, g.prm, flags, 1.0, 0, 1, g.stream, 0, rest, mf))
+        if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, true), flags, 1.0, 0, 1, g.stream, 0, rest, mf))
             return fail("residual kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         cell0 += (long long)b.d.nx * b.d.ny * b.d.nz;
     }
@@ -1243,7 +1253,7 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
                 dim3 tb(32, 4, 2);
                 dim3 gr((d.NI + 31) / 32, (d.NJ + 3) / 4, (pHi - pLo + 2) / 2);
                 KT_BEGIN(K_PREP, sF);
-                launch_pdl(k_prep, gr, tb, sF, d, b.dev, 1, 1, 0, pLo, pHi);
+                launch_pdl(k_prep, gr, tb, sF, d, b.dev, 1, 1, 0, pLo, pHi, residual_discr(1, true), 1);
                 KT_END(K_PREP, sF);
             }
             // residual rows of the k chunks whose +-2 plane stencil is complete
@@ -1306,7 +1316,7 @@ static int form_function_pipelined(const double* wVec, double* rVec, long long n
     if (!ff_pinned(wVec) || !ff_pinned(rVec)) return -1;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
-        if (!b.haveMetrics || b.nOrphans || !tile_kernel_applies(b.d, b.dev, g.prm) || b.d.nz < 16) return -1;
+        if (!b.haveMetrics || b.nOrphans || !tile_kernel_applies(b.d, b.dev, residual_discr(1, true)) || b.d.nz < 16) return -1;
     }
     if (!g_ffIn) {
         CK(cudaStreamCreateWithFlags(&g_ffIn, cudaStreamNonBlocking));
@@ -1409,7 +1419,7 @@ static int mffd_core(long long need, double h) {
     { const char* e = getenv("ADFB_MFFD_FUSED"); if (e && e[0] == '1') fuse = true; }
     if (g_kt.on) fuse = false;
     for (Block& b : g.blocks)
-        if (b.alive && b.level == 1 && !tile_kernel_applies(b.d, b.dev, g.prm)) fuse = false;
+        if (b.alive && b.level == 1 && !tile_kernel_applies(b.d, b.dev, residual_discr(1, true))) fuse = false;
     if (overset_present(1)) fuse = false;   // the exchange rewrites owned fringe cells: p, rhoE must follow (k_etot_owned)
     if (fuse) {
         if (!g.dMffd) {
@@ -1488,7 +1498,7 @@ int adfb_reference_shock_sensor(int level) {
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         KT_BEGIN(K_MISC, g.stream);
-        k_shock<<<(unsigned)((b.d.N + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev);
+        k_shock<<<(unsigned)((b.d.N + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, residual_discr(level, true));
         KT_END(K_MISC, g.stream);
     }
     CK(cudaGetLastError());
@@ -1507,17 +1517,25 @@ int adfb_apply_bcs(int level, int secondHalo, int withTurb) {
     return 0;
 }
 
-// timeStep(onlyRadii), src/solver/solverUtils.F90:43-355 (fine level, directional scaling)
+// timeStep(onlyRadii), src/solver/solverUtils.F90:43-355 (timeStep_block).  The radii are needed only when the residual of
+// the level reads them, i.e. with scalar dissipation: spaceDiscr up to the ground level, spaceDiscrCoarse above it
+// (radiiNeededFine / radiiNeededCoarse, inputParamRoutines.F90:2829-2833).  Otherwise an only-radii call returns at once and
+// leaves the radii of the last full call; the residual of a coarse ground level with fine = matrix or upwind and coarse =
+// scalar reads exactly those.  dirScaling is off unless spaceDiscr is scalar dissipation (:2824).
 int adfb_timestep(int level, int onlyRadii) {
     ADFB_RANGE("adfb_timestep");
     NEED_INIT();
     if (!g.havePrm) return fail("adfb_timestep: adfb_set_params has not been called");
+    const bool above = above_ground(level);
+    const bool radiiNeeded = (above ? g.prm.spaceDiscrCoarse : g.prm.spaceDiscr) == ADFB_DISS_SCALAR;
+    if (onlyRadii && !radiiNeeded) return 0;
+    const int scaleRad = !above && g.prm.spaceDiscr == ADFB_DISS_SCALAR;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         dim3 tb(32, 4, 2);
         dim3 gr((b.d.NI + 31) / 32, (b.d.NJ + 3) / 4, (b.d.NK + 1) / 2);
         KT_BEGIN(K_PREP, g.stream);
-        launch_pdl(k_prep, gr, tb, g.stream, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, 0, INT_MAX);
+        launch_pdl(k_prep, gr, tb, g.stream, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, 0, INT_MAX, residual_discr(level, false), scaleRad);
         KT_END(K_PREP, g.stream);
     }
     CK(cudaGetLastError());
@@ -1535,7 +1553,8 @@ static int adfb_smoother_residual_body(int level, int rkStage) {
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         // coarse level: initRes starts from the residual forcing term (dw = wr)
-        if (launch_residual_core(b.d, b.dev, g.prm, ADFB_RES_FLOW, rFil, 1, 0, g.stream, above_ground(level) ? g.mgInitWr : 0))
+        if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, false), ADFB_RES_FLOW, rFil, 1, 0, g.stream,
+                                 above_ground(level) ? g.mgInitWr : 0))
             return fail("residual launch failed");
         // the primitive <-> conservative round trip that inviscidDissFluxScalarCoarse leaves on w (the matrix form does not convert)
         if (above_ground(level) && fabs(rFil) >= 1.e-10 && g.prm.spaceDiscrCoarse == ADFB_DISS_SCALAR) launch_mg_cells1(b.d, b.dev, 2, g.stream);
@@ -2150,7 +2169,7 @@ int adfb_mg_prolong(int fineLevel) {
 
 // iteration%groundLevel of the solver loop `do groundLevel = mgStartlevel, 1, -1` (solvers.F90:63): the finest level of the
 // multigrid cycles that follow.  Levels above it take the coarse-level branches; the ground level itself runs the fine-grid
-// routines with cflCoarse (currentLevel /= 1) and the coarse discretisation, which must be the fine one here.
+// routines with cflCoarse (currentLevel /= 1), in the discretisation residual_discr picks for the entry point.
 int adfb_set_ground_level(int level) {
     ADFB_RANGE("adfb_set_ground_level");
     NEED_INIT();
@@ -2158,8 +2177,6 @@ int adfb_set_ground_level(int level) {
     bool have = false;
     for (Block& b : g.blocks) if (b.alive && b.level == level) have = true;
     if (!have) return fail("adfb_set_ground_level: no block of level %d", level);
-    if (level > 1 && g.havePrm && g.prm.spaceDiscrCoarse != g.prm.spaceDiscr)
-        return fail("adfb_set_ground_level: a coarse ground level needs spaceDiscrCoarse == spaceDiscr (the kernels read one discretisation)");
     CK(cudaStreamSynchronize(g.stream));
     g.groundLevel = level;
     for (Block& b : g.blocks) if (b.alive) b.dev.coarse = b.level > level ? 1 : 0;

@@ -78,7 +78,10 @@ __global__ void __launch_bounds__(256) k_geom(Dims d, BlockDev b) {
 // part: 0 = every box cell, 1 = owned cells without a halo neighbour (3:nx, ...: the pressure switch of dtl reads the six
 // neighbours), 2 = the rest (the first part does not need the BCs and runs beside them, see residual_body)
 // kOff / kTop: the planes kOff .. kTop only (slab pipeline of adfb_form_function); 0 / INT_MAX: all of them
-__global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, int doRad, int part, int kOff, int kTop) {
+// disc: the discretisation of the residual that reads ss (residual_discr); scaleRad: directional scaling of the radii
+// (doScaling of timeStep: always on the blockette path, dirScaling .and. currentLevel <= groundLevel on the block path)
+__global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, int doRad, int part, int kOff, int kTop, int disc,
+                                              int scaleRad) {
     ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_pdl)
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int j = blockIdx.y * blockDim.y + threadIdx.y;
@@ -94,7 +97,7 @@ __global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, 
     const double rho = b.w[c], p = b.p[c];
     // p / rho**gamma as p*exp(-gamma*log(rho)): |gamma*log(rho)| = O(1), so the result agrees
     // with pow() to a few ulp at less than half the FP64 instructions
-    if (c_prm.spaceDiscr == ADFB_DISS_SCALAR) b.ss[c] = (c_prm.equations == ADFB_EULER) ? p : p * exp(-gam * log(rho));
+    if (disc == ADFB_DISS_SCALAR) b.ss[c] = (c_prm.equations == ADFB_EULER) ? p : p * exp(-gam * log(rho));
     if (i < 1 || i > d.ie || j < 1 || j > d.je || k < 1 || k > d.ke) return;
     const bool viscous = c_prm.equations != ADFB_EULER;
     if (viscous) b.aa[c] = gam * p / rho;
@@ -116,7 +119,7 @@ __global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, 
     double rj = 0.5 * (fabs(ux * sxj + uy * syj + uz * szj) + asf * sqrt(cc2 * s2j));
     double rk = 0.5 * (fabs(ux * sxk + uy * syk + uz * szk) + asf * sqrt(cc2 * s2k));
     double dt = ri + rj + rk;
-    if (b.coarse) {   // doScaling = dirScaling .and. currentLevel <= groundLevel (solverUtils.F90:106)
+    if (!scaleRad) {   // doScaling = dirScaling .and. currentLevel <= groundLevel (solverUtils.F90:106)
         b.radI[c] = ri; b.radJ[c] = rj; b.radK[c] = rk;
     } else {
     ri = dmax_(ri, 1.e-25); rj = dmax_(rj, 1.e-25); rk = dmax_(rk, 1.e-25);
@@ -166,7 +169,7 @@ __global__ void k_param_consts(double* out) {
 // GAOS (experiment switch ADFB_GRAD_AOS=1, main residual path only): the 12 gradients of a node are stored
 // contiguously (96 B) and read back by k_faces with six 128-bit loads per node instead of twelve 64-bit ones
 template <bool GAOS>
-__global__ void __launch_bounds__(NODAL_TPB, NODAL_MINB) k_nodal(Dims d, BlockDev b, int doGrad, int dissApprox) {
+__global__ void __launch_bounds__(NODAL_TPB, NODAL_MINB) k_nodal(Dims d, BlockDev b, int doGrad, int dissApprox, int disc) {
     ADFB_PDL_SYNC();
     const int i = blockIdx.x * blockDim.x + threadIdx.x + 1;
     const int j = blockIdx.y * blockDim.y + threadIdx.y + 1;
@@ -174,14 +177,14 @@ __global__ void __launch_bounds__(NODAL_TPB, NODAL_MINB) k_nodal(Dims d, BlockDe
     if (i > d.ie || j > d.je || k > d.ke) return;
     const int N = (int)d.N, sJ = (int)d.sJ, sK = (int)d.sK;
     const int c = i + sJ * j + sK * k;
-    if (c_prm.spaceDiscr == ADFB_DISS_SCALAR) {
+    if (disc == ADFB_DISS_SCALAR) {
         const double sslim = c_fheat[2];   // 0.001 pInfCorr / rhoInf**gamma (pInfCorr for Euler), k_param_consts
         const double* ss = dissApprox ? b.shock : b.ss;  // *Approx: frozen sensor field (blockette.F90:4385-4396)
         const double s0 = ss[c];
         b.dss[c] = fabs((ss[c + 1] - 2.0 * s0 + ss[c - 1]) / (ss[c + 1] + 2.0 * s0 + ss[c - 1] + sslim));
         b.dss[N + c] = fabs((ss[c + sJ] - 2.0 * s0 + ss[c - sJ]) / (ss[c + sJ] + 2.0 * s0 + ss[c - sJ] + sslim));
         b.dss[2 * N + c] = fabs((ss[c + sK] - 2.0 * s0 + ss[c - sK]) / (ss[c + sK] + 2.0 * s0 + ss[c - sK] + sslim));
-    } else if (c_prm.spaceDiscr == ADFB_DISS_MATRIX) {
+    } else if (disc == ADFB_DISS_MATRIX) {
         // pressure sensor with the omega blend, inviscidDissFluxMatrix blockette.F90:2495-2512
         const double plim = 0.001 * c_prm.pInfCorr;
         const double* p = dissApprox ? b.shock : b.p;  // matrix *Approx uses the frozen sensor (blockette.F90:4655-4670)
@@ -852,12 +855,14 @@ static bool split_faces() {
     if (v < 0) { const char* e = getenv("ADFB_SPLIT_FACES"); v = e ? atoi(e) : 0; }
     return v != 0;
 }
-// true when launch_residual_core hands the flow rows of the full exact residual to the tile kernel
-static bool tile_kernel_applies(const Dims& d, const BlockDev& b, const AdfbParams& prm) {
-    return fused_mode() > 0 && !b.coarse && prm.spaceDiscr == ADFB_DISS_SCALAR && !split_faces();
+// true when launch_residual_core hands the flow rows of the full exact residual in discretisation `disc` to the tile kernel
+static bool tile_kernel_applies(const Dims& d, const BlockDev& b, int disc) {
+    return fused_mode() > 0 && !b.coarse && disc == ADFB_DISS_SCALAR && !split_faces();
 }
 enum { RC_PREP_OWNED = 1, RC_PREP_HALO = 2, RC_SA_INNER = 4, RC_SA_SHELL = 8, RC_FLOW = 16, RC_ALL = 31 };
-static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbParams& prm, unsigned flags, double rFil,
+// disc: the discretisation of this residual (residual_discr in adflow_b200.cu); on a level above the ground level it is
+// spaceDiscrCoarse and selects the first-order coarse-level fluxes
+static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbParams& prm, int disc, unsigned flags, double rFil,
                                 int persistFw, int doRad, cudaStream_t stream, int initWr = 0, int parts = RC_ALL,
                                 MffdEpi mf = MffdEpi{nullptr, 0}) {
     const int flowRes = (flags & ADFB_RES_FLOW) != 0;
@@ -871,7 +876,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     if ((dissApprox || viscApprox) && persistFw) return 1;  // approximate variants exist on the blockette path only
     // experiment switch: AoS nodal-gradient store, only for the exact merged viscous scalar-JST residual (the bench path)
     const bool gradAos = grad_aos() && flowRes && doVisc && !persistFw && !dissApprox && !viscApprox && !b.coarse && !split_faces() &&
-                         !((flags & ADFB_RES_STORE_WALL) != 0) && prm.spaceDiscr == ADFB_DISS_SCALAR;
+                         !((flags & ADFB_RES_STORE_WALL) != 0) && disc == ADFB_DISS_SCALAR;
     dim3 tb(32, 4, 2);
     // The SA row reads only the state and static geometry and writes dw(itu1); the flow rows write dw(1:5).
     // The two chains are independent, so k_sa is forked onto a side stream (also inside graph capture) and
@@ -913,7 +918,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         const int prepPart = ((parts & RC_PREP_OWNED) && (parts & RC_PREP_HALO)) ? 0 : (parts & RC_PREP_OWNED) ? 1 : 2;
         dim3 g((d.NI + tb.x - 1) / tb.x, (d.NJ + tb.y - 1) / tb.y, (d.NK + tb.z - 1) / tb.z);
         KT_BEGIN(K_PREP, stream);
-        launch_pdl(k_prep, g, tb, stream, d, b, updateDt, doRad, prepPart, 0, INT_MAX);
+        launch_pdl(k_prep, g, tb, stream, d, b, updateDt, doRad, prepPart, 0, INT_MAX, disc, (int)!b.coarse);
         KT_END(K_PREP, stream);
     }
     // tile kernel (fused_kernels.cuh): exact central + scalar-JST (+ viscous) flow rows in one launch
@@ -925,7 +930,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     if (fusedSmoother < 0) { const char* e = getenv("ADFB_FUSED_SMOOTHER"); fusedSmoother = e ? atoi(e) : 0; }
     // ADFB_FUSED_SMOOTHER: 1 = the tile kernel for every smoother residual, 2 = only for the stages that form the dissipative and viscous
     // fluxes (rFil /= 0); the central-only stages keep k_faces + k_div, which are cheaper there
-    if (flowRes && fused_mode() > 0 && (!persistFw || fusedSmoother == 1 || (fusedSmoother == 2 && doDiss)) && !b.coarse && prm.spaceDiscr == ADFB_DISS_SCALAR && !dissApprox && !viscApprox && !initWr &&
+    if (flowRes && fused_mode() > 0 && (!persistFw || fusedSmoother == 1 || (fusedSmoother == 2 && doDiss)) && !b.coarse && disc == ADFB_DISS_SCALAR && !dissApprox && !viscApprox && !initWr &&
         !(flags & ADFB_RES_STORE_WALL) && !split_faces()) {
         KT_BEGIN(K_RESID, stream);
         const int rc = launch_flowres_tile(d, b, prm, (int)((b.p - b.w) / d.N), rFil, doDiss, !persistFw, persistFw, stream, mf);
@@ -938,8 +943,8 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         dim3 tn = tune_block("ADFB_NODAL_BLOCK", dim3(32, 4, 2));
         dim3 g((d.ie + tn.x - 1) / tn.x, (d.je + tn.y - 1) / tn.y, (d.ke + tn.z - 1) / tn.z);
         KT_BEGIN(K_NODAL, stream);
-        if (gradAos) launch_pdl(k_nodal<true>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox);
-        else launch_pdl(k_nodal<false>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox);
+        if (gradAos) launch_pdl(k_nodal<true>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
+        else launch_pdl(k_nodal<false>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
         KT_END(K_NODAL, stream);
     }
     if (flowRes && !fusedDone) {
@@ -950,8 +955,8 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
 #define ADFB_LAUNCH_FACES(V, M, D, A) launch_pdl(k_faces<V, M, D, A>, g, tr, stream, d, b, rFil, doVisc, doDiss)
 #define ADFB_FACES_DISC(V, M, A)                                           \
     do {                                                                   \
-        if (prm.spaceDiscr == ADFB_DISS_SCALAR) ADFB_LAUNCH_FACES(V, M, ADFB_DISS_SCALAR, A); \
-        else if (prm.spaceDiscr == ADFB_DISS_MATRIX) ADFB_LAUNCH_FACES(V, M, ADFB_DISS_MATRIX, A); \
+        if (disc == ADFB_DISS_SCALAR) ADFB_LAUNCH_FACES(V, M, ADFB_DISS_SCALAR, A); \
+        else if (disc == ADFB_DISS_MATRIX) ADFB_LAUNCH_FACES(V, M, ADFB_DISS_MATRIX, A); \
         else ADFB_LAUNCH_FACES(V, M, ADFB_UPWIND, A);                       \
     } while (0)
         const int approx = dissApprox | (viscApprox << 1);
@@ -959,10 +964,10 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         const bool storeWall = (flags & ADFB_RES_STORE_WALL) && viscous && doVisc && merged && approx == 0;
         if (b.coarse) {   // coarse multigrid level: first-order scalar dissipation, block path only
             if (merged || approx) return 1;
-            if (prm.spaceDiscrCoarse == ADFB_UPWIND) {   // inviscidUpwindFlux(fineGrid = .false.): first-order states, fluxes.F90:1532
+            if (disc == ADFB_UPWIND) {   // inviscidUpwindFlux(fineGrid = .false.): first-order states, fluxes.F90:1532
                 if (viscous) launch_pdl(k_faces<true, false, ADFB_UPWIND, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
                 else launch_pdl(k_faces<false, false, ADFB_UPWIND, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-            } else if (prm.spaceDiscrCoarse == ADFB_DISS_SCALAR) {
+            } else if (disc == ADFB_DISS_SCALAR) {
                 if (viscous) launch_pdl(k_faces<true, false, ADFB_DISS_SCALAR, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
                 else launch_pdl(k_faces<false, false, ADFB_DISS_SCALAR, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
             } else {
@@ -970,15 +975,15 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
                 else launch_pdl(k_faces<false, false, ADFB_DISS_MATRIX, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
             }
         } else if (storeWall) {  // exact viscous flux + viscSubface%tau/%q planes for the force integration
-            if (prm.spaceDiscr == ADFB_DISS_SCALAR) launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-            else if (prm.spaceDiscr == ADFB_DISS_MATRIX) launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+            if (disc == ADFB_DISS_SCALAR) launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+            else if (disc == ADFB_DISS_MATRIX) launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
             else launch_pdl(k_faces<true, true, ADFB_UPWIND, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
         } else if (approx == 0 && viscous && merged && doVisc && split_faces()) {
             // two launches with fewer registers each (ADFB_SPLIT_FACES=1): central + dissipation, then viscous
-            if (prm.spaceDiscr == ADFB_DISS_SCALAR) {
+            if (disc == ADFB_DISS_SCALAR) {
                 launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
                 launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 2>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-            } else if (prm.spaceDiscr == ADFB_DISS_MATRIX) {
+            } else if (disc == ADFB_DISS_MATRIX) {
                 launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
                 launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 2>, g, tr, stream, d, b, rFil, doVisc, doDiss);
             } else {

@@ -83,13 +83,13 @@ __global__ void __launch_bounds__(256) k_state_prep(Dims d, BlockDev b, int incl
     b.rev[c] = chi3 / (chi3 + cv13) * rnuSA;
 }
 
-// referenceShockSensor (src/adjoint/adjointUtils.F90:1900-1950)
-__global__ void __launch_bounds__(256) k_shock(Dims d, BlockDev b) {
+// referenceShockSensor (src/adjoint/adjointUtils.F90:1900-1950); disc: the discretisation of the residual that reads it
+__global__ void __launch_bounds__(256) k_shock(Dims d, BlockDev b, int disc) {
     const long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= d.N) return;
     const double p = b.p[c];
     // pressure for Euler and for matrix dissipation, entropy otherwise (adjointUtils.F90:1930-1947)
-    b.shock[c] = (c_prm.equations == ADFB_EULER || c_prm.spaceDiscr == ADFB_DISS_MATRIX) ? p : p / pow(b.w[c], c_prm.gammaInf);
+    b.shock[c] = (c_prm.equations == ADFB_EULER || disc == ADFB_DISS_MATRIX) ? p : p / pow(b.w[c], c_prm.gammaInf);
 }
 
 // computeEtotBlock(2,il,2,jl,2,kl) (src/utils/flowUtils.F90:551-672, cpConstant)

@@ -271,9 +271,12 @@ class ADFLOW_B200:
     def fullMultigridStartUp(self, mg_start_level, n_cycles_coarse, cycle="sg", smoother="RK", n_subiterations=1):
         """The full-multigrid start-up of `solver` (src/solver/solvers.F90:63-117): nCyclesCoarse cycles of executeMGCycle on
         every ground level mgStartlevel, ..., 2 (fmgSchedule), each followed by transferToFineGrid(.false.); leaves the ground
-        level at 1."""
+        level at 1.  Each ground level starts like solveState (solvers.F90:1014-1018): the full residual (blocketteRes, in
+        spaceDiscr), then timeStep(.false.); the first smoothing step of the first cycle consumes that residual."""
         for ground, spec in self.fmgSchedule(mg_start_level, cycle):
             self.setGroundLevel(ground)
+            self.residual(RES_FLOW | RES_TURB, level=ground)
+            self.timeStep(False, level=ground)
             cyc = self.cycleStrategy(spec)
             for _ in range(n_cycles_coarse):
                 self.mgCycle(cyc, smoother, n_subiterations)

@@ -283,7 +283,9 @@ int adfb_halo_exchange(int level, int start, int end, int commPressure, int comm
    bcTurbTreatment + applyAllTurbBCThisBlock (src/turbulence/turbBCRoutines.F90:49,662) */
 int adfb_apply_bcs(int level, int secondHalo, int withTurb);
 /* timeStep(onlyRadii): spectral radii radI/J/K and local time step dtl
-   (src/solver/solverUtils.F90:43-355) */
+   (src/solver/solverUtils.F90:43-355).  onlyRadii = 1 does nothing unless the residual of the level reads the radii
+   (scalar dissipation: spaceDiscr up to the ground level, spaceDiscrCoarse above it), as in the reference; the radii
+   are scaled directionally only up to the ground level and only with spaceDiscr = scalar dissipation (dirScaling). */
 int adfb_timestep(int level, int onlyRadii);
 /* `initres(1,nwf); sourceTerms; residual` as called by the smoothers
    (src/solver/smoothers.F90:73-75, src/solver/multiGrid.F90:883-888): block-path
@@ -388,7 +390,9 @@ int adfb_mg_prolong(int fineLevel);
 /* Full-multigrid start-up, the solver loop `do groundLevel = mgStartlevel, 1, -1` (src/solver/solvers.F90:63-117):
    adfb_set_ground_level = iteration%groundLevel, the finest level of the cycles that follow (levels above it take the
    coarse-level branches; a coarse ground level runs the fine-grid routines with cflCoarse and second halos, and needs
-   spaceDiscrCoarse == spaceDiscr and second-level halo lists for that level);
+   second-level halo lists for that level).  Any pair of spaceDiscr and spaceDiscrCoarse: on a coarse ground level
+   adfb_residual (blocketteRes) uses spaceDiscr, the smoother and multigrid entry points the fine-grid routines of
+   spaceDiscrCoarse (residual_block with currentLevel /= 1);
    adfb_mg_prolong_solution = transferToFineGrid(corrections = .false.) (multiGrid.F90:326-654) with extrapolateSolution
    (:656-737) and extrapolateViscosities (:739-823): the solution of ground level fineLevel + 1 interpolated to fineLevel,
    halos extrapolated, turbulence + flow BCs and the exchanges as the reference orders them.  Lower the ground level
