@@ -99,6 +99,7 @@ struct Context {
     // CUDA graphs of whole entry points (launch-latency bound sequences of small kernels)
     std::map<unsigned long long, cudaGraphExec_t> graphs;
     std::map<unsigned long long, long long> graphLaunches;
+    std::vector<unsigned long long> ffKeys;   // graphs of the pipelined form function, oldest first (at most 8 kept)
     bool useGraphs = true;
     bool capturing = false;
     // ANK (module ANKSolver): options, per-cell time-step blocks, the perturbed vector of the last product
@@ -284,6 +285,7 @@ void drop_graphs() {
     for (auto& kv : g.graphs) cudaGraphExecDestroy(kv.second);
     g.graphs.clear();
     g.graphLaunches.clear();
+    g.ffKeys.clear();
 }
 
 }  // namespace
@@ -369,6 +371,9 @@ int adfb_finalize(void) {
     for (double** p : {&g.ankT, &g.ankPert, &g.kryV, &g.kryRed}) { if (*p) cudaFree(*p); *p = nullptr; }
     g.ankTN = 0; g.ankPertN = 0; g.kryVN = 0;
     g.haveAnk = false; g.ankHaveT = false; g.ankHaveBase = false;
+    // so do the parameters and the multigrid position: a later context starts on ground level 1 and must set its parameters
+    g.havePrm = false;
+    g.groundLevel = 1; g.mgInitWr = 1;
     drop_graphs();
     for (auto* M : {&g.pats, &g.ovPats}) {
         for (auto& kv : *M) for (void* q : kv.second.allocs) cudaFree(q);
@@ -512,6 +517,8 @@ int adfb_block_set_geometry(int blk, const double* x, const double* si, const do
                             const double* vol, const double* volRef, const double* d2Wall, const int8_t* porI,
                             const int8_t* porJ, const int8_t* porK, const int32_t* iblank) {
     NEED_INIT();
+    // No drop_graphs: a mesh warp rewrites the block's geometry arrays in place, and the cached graphs hold only their
+    // addresses and the block extents, which do not change (the same holds for the state uploads).
     Block* b = get_block(blk);
     if (!b) return fail("adfb_block_set_geometry: no block %d", blk);
     if (!x || !vol || !volRef || !porI || !porJ || !porK || !iblank)
@@ -1334,7 +1341,7 @@ static int form_function_pipelined(const double* wVec, double* rVec, long long n
         h = (h ^ v) * 1099511628211ull;
     const unsigned long long key = (12ull << 40) | (h & 0xffffffffffull);
     {   // a handful of vector pairs at most: forget the oldest graph beyond that
-        static std::vector<unsigned long long> keys;
+        std::vector<unsigned long long>& keys = g.ffKeys;
         if (std::find(keys.begin(), keys.end(), key) == keys.end()) {
             keys.push_back(key);
             if (keys.size() > 8) {
@@ -1716,6 +1723,8 @@ int adfb_ank_set_params(const AdfbAnkParams* ank) {
     if (!(ank->cfl > 0.0) || !(ank->cflLimit > 0.0) || !(ank->turbCFLScale > 0.0)) return fail("adfb_ank_set_params: CFL values must be positive");
     if (ank->charTimeStepType < 0 || ank->charTimeStepType > 2) return fail("adfb_ank_set_params: charTimeStepType %d (0 None, 1 VLR, 2 Turkel)", ank->charTimeStepType);
     if (ank->coupled && g.havePrm && g.prm.equations != ADFB_RANS) return fail("adfb_ank_set_params: coupled ANK needs the RANS equations");
+    // No drop_graphs: the ANK products launch their own kernels with g.ank as an argument at every call, and the residual
+    // they call is keyed by its flags, which carry the ANK options it depends on (ank_res_flags).
     g.ank = *ank;
     g.haveAnk = true; g.ankHaveT = false; g.ankHaveBase = false;
     return 0;

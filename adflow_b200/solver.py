@@ -37,31 +37,40 @@ class ADFLOW_B200:
         blk = len(self.blocks)
         d = hb.d
         check(self.L.adfb_block_create(blk, level, d.nx, d.ny, d.nz, hb.nw, int(hb.right_handed)), "adfb_block_create")
+        self.setGeometry(blk, hb, upload_metrics)
+        if hb.subfaces:
+            self.setBCData(blk, hb.subfaces)
+        self.blocks.append(hb)
+        self.uploadState(blk, hb)
+        return blk
+
+    def setGeometry(self, blk, hb, upload_metrics=True):
+        """Upload the geometry of hb to block blk (a mesh warp on a live block); upload_metrics=False: the face
+        metrics are formed from the coordinates on the device."""
         r = hb.ref
         si = r("si") if upload_metrics else None
         sj = r("sj") if upload_metrics else None
         sk = r("sk") if upload_metrics else None
         arrs = [r("x"), si, sj, sk, r("vol"), r("volRef"), r("d2Wall"), r("porI"), r("porJ"), r("porK"), r("iblank")]
         check(self.L.adfb_block_set_geometry(blk, *[ptr(a) for a in arrs]), "adfb_block_set_geometry")
-        if hb.subfaces:
-            n = len(hb.subfaces)
-            sf = (AdfbSubface * n)()
-            keep = []
-            for q, s in enumerate(hb.subfaces):
-                sf[q].bcType, sf[q].faceId = s["bcType"], s["faceId"]
-                sf[q].icBeg, sf[q].icEnd, sf[q].jcBeg, sf[q].jcEnd = s["icBeg"], s["icEnd"], s["jcBeg"], s["jcEnd"]
-                sf[q].subsonicInletTreatment = int(s.get("subsonicInletTreatment", 0))
-                for name in ("norm", "rface", "uSlip", "TNSWall", "ps", "rho", "velx", "vely", "velz", "ptInlet", "ttInlet", "htInlet",
-                             "flowXdirInlet", "flowYdirInlet", "flowZdirInlet", "turbInlet"):
-                    a = s.get(name)
-                    if a is not None:
-                        a = np.asfortranarray(a, dtype=np.float64)
-                        keep.append(a)
-                        setattr(sf[q], name, a.ctypes.data)
-            check(self.L.adfb_block_set_bc(blk, n, sf), "adfb_block_set_bc")
-        self.blocks.append(hb)
-        self.uploadState(blk, hb)
-        return blk
+
+    def setBCData(self, blk, subfaces):
+        """Replace the subfaces of block blk (layout and prescribed BC data)."""
+        n = len(subfaces)
+        sf = (AdfbSubface * max(n, 1))()
+        keep = []
+        for q, s in enumerate(subfaces):
+            sf[q].bcType, sf[q].faceId = s["bcType"], s["faceId"]
+            sf[q].icBeg, sf[q].icEnd, sf[q].jcBeg, sf[q].jcEnd = s["icBeg"], s["icEnd"], s["jcBeg"], s["jcEnd"]
+            sf[q].subsonicInletTreatment = int(s.get("subsonicInletTreatment", 0))
+            for name in ("norm", "rface", "uSlip", "TNSWall", "ps", "rho", "velx", "vely", "velz", "ptInlet", "ttInlet", "htInlet",
+                         "flowXdirInlet", "flowYdirInlet", "flowZdirInlet", "turbInlet"):
+                a = s.get(name)
+                if a is not None:
+                    a = np.asfortranarray(a, dtype=np.float64)
+                    keep.append(a)
+                    setattr(sf[q], name, a.ctypes.data)
+        check(self.L.adfb_block_set_bc(blk, n, sf), "adfb_block_set_bc")
 
     def uploadState(self, blk, hb, with_visc=True):
         check(self.L.adfb_upload_state(blk, ptr(hb.w), ptr(hb.p)), "adfb_upload_state")
@@ -382,6 +391,10 @@ class ADFLOW_B200:
 
     def launchCount(self):
         return int(self.L.adfb_launch_count())
+
+    def graphCount(self):
+        """CUDA graphs cached by the context (-1: graphs are off)"""
+        return int(self.L.adfb_graph_count())
 
     def close(self):
         self.L.adfb_finalize()
