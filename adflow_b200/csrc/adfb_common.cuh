@@ -160,6 +160,16 @@ struct KTimer {
 };
 static KTimer g_kt;
 
+// What the launch helpers need of the context: properties of the device it is bound to and the side stream of the SA row.
+// adfb_init reads and creates them for the device it binds, adfb_finalize releases them.
+struct LaunchEnv {
+    int nSM = 0;                 // multiprocessors
+    size_t smemOptin = 0;        // opt-in dynamic shared memory per CTA
+    // the SA row of the residual runs here beside the flow rows (launch_residual_core)
+    cudaStream_t saStream = nullptr;
+    cudaEvent_t saFork = nullptr, saJoin = nullptr;
+};
+
 // lanes per line for the partitioned Thomas kernels (tridiag_part.cuh): 8 lanes x <= 16 rows, 16 lanes x <= 16
 // rows, or 0 = one thread per line (short or very long lines).
 static inline int adfb_part_lanes(int nl) {

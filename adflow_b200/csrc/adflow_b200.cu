@@ -37,7 +37,6 @@ struct Block {
     std::vector<void*> allocs;
     bool haveMetrics = false;
     std::vector<AdfbSubface> subfaces;  // host copies (device arrays in bcDev)
-    size_t slabBytes = 0;               // w, p, rlv, rev slab
     std::vector<void*> bcAllocs;
     // multigrid: the next finer / coarser block of the same mesh block and the transfer tables (on the coarse
     // block: mg?Fine, mg?Weight; the fine block's mg?Coarse are kept with the coarse block as well)
@@ -54,6 +53,14 @@ struct Context {
     bool ready = false;
     int device = -1, rank = 0, nranks = 1;
     cudaStream_t stream = nullptr;
+    LaunchEnv env;
+    // halo exchange split around the BCs (multi-rank): pack and send / receive run on commStream
+    cudaStream_t commStream = nullptr;
+    cudaEvent_t evPost = nullptr, evDone = nullptr;
+    // slab pipeline of the form function: copies in, copies out, back end of a slab; [0..2][slab] and [3][fork / join]
+    cudaStream_t ffIn = nullptr, ffOut = nullptr, ffBack = nullptr;
+    cudaEvent_t ffEv[4][34] = {};
+    double* dConst = nullptr;   // parameter constants formed on the device (adfb_set_params)
     AdfbParams prm;
     bool havePrm = false;
     std::vector<Block> blocks;
@@ -288,6 +295,31 @@ void drop_graphs() {
     g.ffKeys.clear();
 }
 
+// The streams, events and buffers of the context, for the device that is current.  The library stream carries the
+// latency-bound chains (BC levels, line solves) at the highest priority, and so does the stream of the SA row forked beside
+// the flow rows: that is the priority the SA row has run and been measured at (cudaStreamCopyAttributes from the library
+// stream, which carries the priority attribute, used to precede every fork).
+int create_device_resources() {
+    int prLo = 0, prHi = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&prLo, &prHi));
+    for (cudaStream_t* s : {&g.stream, &g.env.saStream}) CK(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, prHi));
+    for (cudaStream_t* s : {&g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) CK(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
+    for (cudaEvent_t* e : {&g.env.saFork, &g.env.saJoin, &g.evPost, &g.evDone}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    for (auto& row : g.ffEv) for (cudaEvent_t& e : row) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CK(cudaMalloc((void**)&g.dConst, 8 * sizeof(double)));
+    CK(cudaMallocHost((void**)&g.hRed, 256 * sizeof(double)));
+    return 0;
+}
+void release_device_resources() {
+    for (cudaEvent_t* e : {&g.env.saFork, &g.env.saJoin, &g.evPost, &g.evDone}) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
+    for (auto& row : g.ffEv) for (cudaEvent_t& e : row) { if (e) cudaEventDestroy(e); e = nullptr; }
+    for (cudaStream_t* s : {&g.stream, &g.env.saStream, &g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) { if (*s) cudaStreamDestroy(*s); *s = nullptr; }
+    if (g.dConst) cudaFree(g.dConst);
+    g.dConst = nullptr;
+    if (g.hRed) cudaFreeHost(g.hRed);
+    g.hRed = nullptr;
+}
+
 }  // namespace
 
 // ===========================================================================
@@ -322,18 +354,30 @@ int adfb_init(int device, const void* ncclUniqueId, int rank, int nranks) {
         return fail("adfb_init: no CUDA device available (%s); this library has no CPU path",
                     e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
     if (device < 0 || device >= n) return fail("adfb_init: device %d out of range (0..%d)", device, n - 1);
+    // the streams, events and buffers belong to the device they were created on
+    if (g.stream && device != g.device)
+        return fail("adfb_init: the context is bound to device %d; adfb_finalize it before binding device %d", g.device, device);
     CK(cudaSetDevice(device));
     if (!g.stream) {
-        // the library stream carries the latency-bound chains (BC levels, line solves): highest priority, so that work forked onto
-        // side streams (SA row, overlap experiments: default = lowest priority) never delays them (ADFB_STREAM_PRIO=0: default priority)
-        int prLo = 0, prHi = 0;
-        cudaDeviceGetStreamPriorityRange(&prLo, &prHi);
-        const char* e = getenv("ADFB_STREAM_PRIO");
-        const int pr = (e && e[0] == '0') ? prLo : prHi;
-        CK(cudaStreamCreateWithPriority(&g.stream, cudaStreamNonBlocking, pr));
+        if (create_device_resources()) {
+            release_device_resources();
+            return 1;
+        }
+        g.device = device;
+    }
+    {
+        int v = 0;
+        CK(cudaDeviceGetAttribute(&g.env.nSM, cudaDevAttrMultiProcessorCount, device));
+        CK(cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+        g.env.smemOptin = (size_t)v;
+        // the kernels that take more dynamic shared memory than the default 48 KiB
+        for (const void* k : {(const void*)k_flowres<true, true>, (const void*)k_flowres<true, false>, (const void*)k_flowres<false, true>,
+                              (const void*)k_flowres<false, false>})
+            CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+        CK(cudaFuncSetAttribute(k_resavg_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kResavgSmemMax));
+        CK(cudaFuncSetAttribute(k_dadi_thomas_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDadiTileSmem));
     }
     g.device = device; g.rank = rank; g.nranks = nranks;
-    if (!g.hRed) CK(cudaMallocHost((void**)&g.hRed, 256 * sizeof(double)));
     g.err.clear();
     if (g.comm) { g.nccl.CommDestroy(g.comm); g.comm = nullptr; }   // re-init: the previous communicator goes
     if (nranks > 1) {
@@ -353,6 +397,9 @@ int adfb_init(int device, const void* ncclUniqueId, int rank, int nranks) {
 
 int adfb_finalize(void) {
     if (!g.ready) return 0;
+    // the graphs first: the pipelined form function's graphs hold the context's events
+    drop_graphs();
+    cudaStreamSynchronize(g.stream);
     for (size_t i = 0; i < g.blocks.size(); i++)
         if (g.blocks[i].alive) adfb_block_destroy((int)i);
     g.blocks.clear();
@@ -360,8 +407,6 @@ int adfb_finalize(void) {
     g.dRed = nullptr; g.dRedN = 0;
     if (g.dMffd) { cudaFree(g.dMffd); g.dMffd = nullptr; }
     if (g.hMffd) { cudaFreeHost(g.hMffd); g.hMffd = nullptr; }
-    if (g.hRed) cudaFreeHost(g.hRed);
-    g.hRed = nullptr;
     if (g.dVec) cudaFree(g.dVec);
     g.dVec = nullptr; g.dVecN = 0;
     for (double** p : {&g.nkA, &g.nkU, &g.nkF0, &g.nkY}) { if (*p) cudaFree(*p); *p = nullptr; }
@@ -374,14 +419,15 @@ int adfb_finalize(void) {
     // so do the parameters and the multigrid position: a later context starts on ground level 1 and must set its parameters
     g.havePrm = false;
     g.groundLevel = 1; g.mgInitWr = 1;
-    drop_graphs();
     for (auto* M : {&g.pats, &g.ovPats}) {
         for (auto& kv : *M) for (void* q : kv.second.allocs) cudaFree(q);
         M->clear();
     }
     if (g.comm) { g.nccl.CommDestroy(g.comm); g.comm = nullptr; }
-    if (g.stream) cudaStreamDestroy(g.stream);
-    g.stream = nullptr;
+    release_device_resources();
+    g_kt.collect();
+    for (cudaEvent_t e : g_kt.pool) cudaEventDestroy(e);
+    g_kt.pool.clear();
     g.ready = false;
     return 0;
 }
@@ -430,17 +476,15 @@ int adfb_set_params(const AdfbParams* prm) {
     g.havePrm = true;
     CK(cudaMemcpyToSymbolAsync(c_prm, &g.prm, sizeof(AdfbParams), 0, cudaMemcpyHostToDevice, g.stream));
     {
-        static double fheat[16];
+        double fheat[16] = {};
         const double gm1 = g.prm.gammaInf - 1.0;
         fheat[0] = 1.0 / (g.prm.prandtl * gm1); fheat[1] = 1.0 / (g.prm.prandtlTurb * gm1);
         fheat[3] = 1.0 / g.prm.rsaCb3; fheat[4] = 1.0 / (g.prm.rsaK * g.prm.rsaK);
         fheat[7] = 1.0 / gm1; fheat[8] = 0.000001 * g.prm.gammaInf * g.prm.pInfCorr / g.prm.rhoInf;
         CK(cudaMemcpyToSymbolAsync(c_fheat, fheat, sizeof fheat, 0, cudaMemcpyHostToDevice, g.stream));
-        static double* dConst = nullptr;
-        if (!dConst) CK(cudaMalloc((void**)&dConst, 8 * sizeof(double)));
-        k_param_consts<<<1, 1, 0, g.stream>>>(dConst);   // reads the c_prm uploaded above (stream order)
-        CK(cudaMemcpyToSymbolAsync(c_fheat, dConst, sizeof(double), 2 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-        CK(cudaMemcpyToSymbolAsync(c_fheat, dConst + 1, 2 * sizeof(double), 5 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
+        k_param_consts<<<1, 1, 0, g.stream>>>(g.dConst);   // reads the c_prm uploaded above (stream order)
+        CK(cudaMemcpyToSymbolAsync(c_fheat, g.dConst, sizeof(double), 2 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
+        CK(cudaMemcpyToSymbolAsync(c_fheat, g.dConst + 1, 2 * sizeof(double), 5 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
         CK(cudaStreamSynchronize(g.stream));
     }
     {
@@ -468,11 +512,9 @@ int adfb_block_create(int blk, int level, int nx, int ny, int nz, int nw, int ri
     BlockDev& v = b.dev;
     memset(&v, 0, sizeof v);
     int rc = 0;
-    // state slab: w(nw), p, rlv, rev contiguous, so that one L2 access-policy window can cover the arrays every kernel of
-    // a step re-reads (set_l2_window below, off by default)
+    // state slab: w(nw), p, rlv, rev contiguous (the tile kernel loads it through one tensor map)
     rc |= dalloc(b, &v.w, N * (nw + 3));
     v.p = v.w + N * nw; v.rlv = v.p + N; v.rev = v.rlv + N;
-    b.slabBytes = (size_t)N * (nw + 3) * sizeof(double);
     rc |= dalloc(b, &v.x, N * 3); rc |= dalloc(b, &v.si, N * 3); rc |= dalloc(b, &v.sj, N * 3); rc |= dalloc(b, &v.sk, N * 3);
     rc |= dalloc(b, &v.vol, N); rc |= dalloc(b, &v.volRef, N); rc |= dalloc(b, &v.d2Wall, N);
     rc |= dalloc(b, &v.porI, N); rc |= dalloc(b, &v.porJ, N); rc |= dalloc(b, &v.porK, N); rc |= dalloc(b, &v.iblank, N);
@@ -844,8 +886,6 @@ extern "C" int adfb_block_set_orphans(int blk, int nOrphans, const int32_t* orph
 //                run the grouped ncclSend/ncclRecv on the communication stream
 //   2 "finish" : join the communication stream, same-rank copies, unpack, then the overset pattern and the owned-cell
 //                total energy -- after the BCs, like the un-split order (edge halos of the BCs read the OLD interface halos)
-static cudaStream_t g_commStream = nullptr;
-static cudaEvent_t g_evPost = nullptr, g_evDone = nullptr;
 static bool halo_split_ok(int level) {
     static int on = -1;
     if (on < 0) { const char* e = getenv("ADFB_HALO_OVERLAP"); on = e ? atoi(e) : 1; }
@@ -860,11 +900,6 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
     Context::Pattern* both[2] = {nullptr, nullptr};
     { auto it = g.pats.find(level); if (it != g.pats.end()) both[0] = &it->second; }
     { auto it = g.ovPats.find(level); if (it != g.ovPats.end()) both[1] = &it->second; }
-    if (phase && !g_commStream) {
-        CK(cudaStreamCreateWithFlags(&g_commStream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&g_evPost, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&g_evDone, cudaEventDisableTiming));
-    }
     for (Context::Pattern* PP : both) {
         if (!PP) continue;
         Context::Pattern& P = *PP;
@@ -873,10 +908,10 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
         if (phase == 1 && !oneToOne) continue;           // the overset pattern is exchanged in one piece by "finish"
         const bool doPost = phase == 0 || phase == 1 || !oneToOne;      // pack + send/recv
         const bool doFinish = phase == 0 || phase == 2;                  // local copies + unpack
-        cudaStream_t cs = (phase == 1) ? g_commStream : g.stream;        // stream of pack + NCCL
+        cudaStream_t cs = (phase == 1) ? g.commStream : g.stream;        // stream of pack + NCCL
         if (phase == 1) {
-            CK(cudaEventRecord(g_evPost, g.stream));
-            CK(cudaStreamWaitEvent(g_commStream, g_evPost, 0));
+            CK(cudaEventRecord(g.evPost, g.stream));
+            CK(cudaStreamWaitEvent(g.commStream, g.evPost, 0));
         }
         if ((int)g.blocks.size() != P.tabBlocks) return fail("halo exchange: blocks changed after adfb_comm_set_pattern");
         const int key = start | (end << 4) | ((commPressure ? 1 : 0) << 8) | ((commViscous ? 1 : 0) << 9);
@@ -935,8 +970,8 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
             const int rc2 = g.nccl.GroupEnd();
             if (rc != 0 || rc2 != 0) return fail("NCCL halo exchange: %s", g.nccl.GetErrorString(rc ? rc : rc2));
         }
-        if (phase == 1) { CK(cudaEventRecord(g_evDone, g_commStream)); continue; }
-        if (phase == 2 && oneToOne) CK(cudaStreamWaitEvent(g.stream, g_evDone, 0));
+        if (phase == 1) { CK(cudaEventRecord(g.evDone, g.commStream)); continue; }
+        if (phase == 2 && oneToOne) CK(cudaStreamWaitEvent(g.stream, g.evDone, 0));
         if (!doFinish) continue;
         if (P.nInt) {
             const long long n = P.nInt * nVar;
@@ -992,7 +1027,6 @@ int adfb_halo_exchange(int level, int start, int end, int commPressure, int comm
 }
 
 static int residual_body(int level, unsigned flags);
-static void set_l2_window();
 // an overset pattern with entries exists on this level: whalo2 then really changes rhoE of fringe cells
 // (computeEtotBlock after wOverset, haloExchange.F90:174-197), so the owned-cell etot pass is not idempotent
 static bool overset_present(int level) {
@@ -1007,79 +1041,15 @@ int adfb_residual(int level, unsigned flags) {
     for (Block& b : g.blocks)
         if (b.alive && b.level == level && !b.haveMetrics) return fail("adfb_residual: geometry of a block was never set");
     const unsigned long long key = (1ull << 40) | ((unsigned long long)level << 32) | flags | (g.mffdFuse ? (1ull << 31) : 0ull);
-    set_l2_window();
     return run_graphed(key, [&]() { return residual_body(level, flags); });
 }
 
-// L2 residency of the state slab: persisting access-policy window on the library stream (inherited by the kernel
-// nodes of captured graphs).  Only when exactly one block lives on the device (one window per stream).
-static void set_l2_window() {
-    static int mode = -1;
-    // Off by default: on H100 (50 MB L2) the C2 slab (37 MB) takes most of the persisting set-aside and starves the streamed
-    // arrays.  C2 on one H100 SXM (400 W limit): residual step 1396 Mcells/s off, 1177 on; 5-stage RK cycle 1.59 ms off,
-    // 2.58 ms on.  ADFB_L2_PERSIST=1 turns it on.
-    if (mode < 0) { const char* e = getenv("ADFB_L2_PERSIST"); mode = e ? atoi(e) : 0; }
-    static const void* current = nullptr;
-    Block* only = nullptr;
-    int nAlive = 0;
-    for (Block& b : g.blocks) if (b.alive) { only = &b; nAlive++; }
-    const void* want = (mode && nAlive == 1) ? (const void*)only->dev.w : nullptr;
-    if (want == current) return;
-    current = want;
-    cudaStreamAttrValue av;
-    memset(&av, 0, sizeof av);
-    if (want) {
-        int dev = 0, maxWin = 0, l2 = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&maxWin, cudaDevAttrMaxAccessPolicyWindowSize, dev);
-        cudaDeviceGetAttribute(&l2, cudaDevAttrMaxPersistingL2CacheSize, dev);
-        size_t bytes = only->slabBytes;
-        if ((size_t)maxWin < bytes) bytes = (size_t)maxWin;
-        cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)l2 < bytes ? (size_t)l2 : bytes);
-        av.accessPolicyWindow.base_ptr = (void*)want;
-        av.accessPolicyWindow.num_bytes = bytes;
-        av.accessPolicyWindow.hitRatio = ((size_t)l2 >= bytes) ? 1.0f : (float)l2 / (float)bytes;
-        av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    } else {
-        av.accessPolicyWindow.num_bytes = 0;
-    }
-    cudaStreamSetAttribute(g.stream, cudaStreamAttributeAccessPolicyWindow, &av);
-    cudaGetLastError();  // a device without the feature just ignores it
-}
-
 static int residual_body(int level, unsigned flags) {
-    // The inner part of k_prep and of the SA row read no halo cell, so they do not have to wait for the boundary conditions
-    // and the exchange: with ADFB_OVERLAP_BC=1 they run on a second stream beside the BC chain and are joined before the
-    // halo-dependent rest.  The small dependent BC launches then queue behind the big kernels' CTAs and the chain gets
-    // longer than the work it hides; off by default.
-    static int overlapOn = -1;
-    if (overlapOn < 0) { const char* e = getenv("ADFB_OVERLAP_BC"); overlapOn = e ? atoi(e) : 0; }
-    static cudaStream_t s2 = nullptr;
-    static cudaEvent_t eFork = nullptr, eJoin = nullptr;
-    const bool preamble = !(flags & ADFB_RES_SKIP_PREAMBLE);
-    // (an overset exchange rewrites p and rhoE of owned fringe cells: nothing may run ahead of it then)
-    const bool overlap = overlapOn && preamble && !g_kt.on && !overset_present(level);
-    if (overlap && !s2) {
-        CK(cudaStreamCreateWithFlags(&s2, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&eFork, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&eJoin, cudaEventDisableTiming));
-    }
-    if (preamble) {
+    if (!(flags & ADFB_RES_SKIP_PREAMBLE)) {
         for (Block& b : g.blocks) {
             if (!b.alive || b.level != level) continue;
             // blocketteRes :213-226: p, rlv, rev on owned cells, then turbulence and flow BCs
             if (!g.mffdFuse && launch_state_prep(b.d, b.dev, g.prm, false, (flags & ADFB_RES_FLOW) != 0, g.stream)) return fail("state prep launch failed");
-        }
-        if (overlap) {
-            CK(cudaEventRecord(eFork, g.stream));
-            CK(cudaStreamWaitEvent(s2, eFork, 0));
-            for (Block& b : g.blocks) {
-                if (!b.alive || b.level != level) continue;
-                if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, true), flags, 1.0, 0, 1, s2, 0, RC_PREP_OWNED | RC_SA_INNER))
-                    return fail("residual kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-            }
-            CK(cudaEventRecord(eJoin, s2));
         }
         // whalo2(1, lStart, lEnd, T, T, T), blockette.F90:231-246; the owned-cell
         // computeEtotBlock of whalo2 is fused into k_state_prep (see DESIGN.md).  Multi-rank: the send lists (owned cells)
@@ -1105,14 +1075,12 @@ static int residual_body(int level, unsigned flags) {
                     return fail("BC launch failed");
             }
         }
-        if (overlap) CK(cudaStreamWaitEvent(g.stream, eJoin, 0));
     }
-    const int rest = overlap ? (RC_PREP_HALO | RC_SA_SHELL | RC_FLOW) : RC_ALL;
     long long cell0 = 0;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         const MffdEpi mf = {g.mffdFuse ? g.dMffd : nullptr, cell0};
-        if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, true), flags, 1.0, 0, 1, g.stream, 0, rest, mf))
+        if (launch_residual_core(b.d, b.dev, g.prm, g.env, residual_discr(level, true), flags, 1.0, 0, 1, g.stream, 0, mf))
             return fail("residual kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
         cell0 += (long long)b.d.nx * b.d.ny * b.d.nz;
     }
@@ -1175,8 +1143,6 @@ static const unsigned kNkFlags = ADFB_RES_FLOW | ADFB_RES_TURB;
 // the host-to-device copy, the kernels and the device-to-host copy of one call overlap (three streams, full-duplex PCIe).
 // Same kernels, same operands as the one-shot path: the result is identical.  Used when both vectors are page-locked, the
 // blocks have no exchange partners (no 1-to-1 / overset pattern on level 1) and the tile kernel applies; ADFB_FF_PIPE=0 disables it.
-static cudaStream_t g_ffIn = nullptr, g_ffOut = nullptr, g_ffBack = nullptr;
-static cudaEvent_t g_ffEv[4][34];
 static bool ff_pinned(const void* p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
@@ -1190,20 +1156,16 @@ static int form_function_pipe_slabs() {   // read at every call: tests switch it
 // cost more host time than the GPU needs for them).  Front end of a slab (setW, p / rlv / rev, BCs, time step / sensor) on the
 // library stream, back end (SA row, tile kernel, setRVec) on a second one: the front end of slab s+1 touches planes above the
 // ones the back end of slab s reads, so the two run side by side.
-static int form_function_pipe_kc() {   // planes per CTA of the tile kernel inside the pipeline
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("ADFB_FF_KC"); v = e ? atoi(e) : 4; if (v < 1) v = 4; }
-    return v;
-}
-static int form_function_pipe_body(const double* wVec, double* rVec, int wantSlabs, int twoStreams) {
-    const int kc = form_function_pipe_kc();
+static const int kFfPlanesPerCta = 4;   // k planes per CTA of the tile kernel inside the pipeline
+static int form_function_pipe_body(const double* wVec, double* rVec, int wantSlabs) {
+    const int kc = kFfPlanesPerCta;
     const bool rans = g.prm.equations == ADFB_RANS;
-    cudaStream_t sF = g.stream, sB = twoStreams ? g_ffBack : g.stream;
+    cudaStream_t sF = g.stream, sB = g.ffBack;
     // fork: the other streams start after whatever the library stream still has in flight
-    CK(cudaEventRecord(g_ffEv[3][0], sF));
-    CK(cudaStreamWaitEvent(g_ffIn, g_ffEv[3][0], 0));
-    CK(cudaStreamWaitEvent(g_ffOut, g_ffEv[3][0], 0));
-    if (twoStreams) CK(cudaStreamWaitEvent(sB, g_ffEv[3][0], 0));
+    CK(cudaEventRecord(g.ffEv[3][0], sF));
+    CK(cudaStreamWaitEvent(g.ffIn, g.ffEv[3][0], 0));
+    CK(cudaStreamWaitEvent(g.ffOut, g.ffEv[3][0], 0));
+    CK(cudaStreamWaitEvent(sB, g.ffEv[3][0], 0));
     long long off = 0;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
@@ -1230,14 +1192,14 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
         auto ownedEnd = [&](int chunkEnd) { return std::min(chunkEnd * kc, d.nz); };   // owned plane index (0-based), exclusive
         for (int q = 0; q < S; q++) {   // all host-to-device copies are queued at once; they run back to back on their stream
             const long long q0 = (long long)ownedEnd(cb[q]) * plane, q1 = (long long)ownedEnd(cb[q + 1]) * plane;
-            CK(cudaMemcpyAsync(g.nkA + off + q0, wVec + off + q0, (size_t)(q1 - q0) * sizeof(double), cudaMemcpyHostToDevice, g_ffIn));
-            CK(cudaEventRecord(g_ffEv[0][q], g_ffIn));
+            CK(cudaMemcpyAsync(g.nkA + off + q0, wVec + off + q0, (size_t)(q1 - q0) * sizeof(double), cudaMemcpyHostToDevice, g.ffIn));
+            CK(cudaEventRecord(g.ffEv[0][q], g.ffIn));
         }
         int cNext = 0;   // first k chunk whose residual has not been formed
         for (int q = 0; q < S; q++) {
             const bool first = q == 0, last = q == S - 1;
             const int o0 = ownedEnd(cb[q]), o1 = ownedEnd(cb[q + 1]);   // owned planes o0 .. o1-1 (0-based) = absolute 2+o0 .. 1+o1
-            CK(cudaStreamWaitEvent(sF, g_ffEv[0][q], 0));
+            CK(cudaStreamWaitEvent(sF, g.ffEv[0][q], 0));
             // setW + p / rlv / rev of the slab's owned cells
             {
                 const long long q0 = (long long)o0 * plane, q1 = (long long)o1 * plane;
@@ -1260,51 +1222,47 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
                 dim3 tb(32, 4, 2);
                 dim3 gr((d.NI + 31) / 32, (d.NJ + 3) / 4, (pHi - pLo + 2) / 2);
                 KT_BEGIN(K_PREP, sF);
-                launch_pdl(k_prep, gr, tb, sF, d, b.dev, 1, 1, 0, pLo, pHi, residual_discr(1, true), 1);
+                launch_pdl(k_prep, gr, tb, sF, d, b.dev, 1, 1, pLo, pHi, residual_discr(1, true), 1);
                 KT_END(K_PREP, sF);
             }
             // residual rows of the k chunks whose +-2 plane stencil is complete
             int cEnd = cNext;
             while (cEnd < nChunks && (last || 2 + ownedEnd(cEnd + 1) - 1 + 2 <= pHi)) cEnd++;
             if (cEnd > cNext) {
-                if (twoStreams) {
-                    CK(cudaEventRecord(g_ffEv[2][q], sF));
-                    CK(cudaStreamWaitEvent(sB, g_ffEv[2][q], 0));
-                }
+                CK(cudaEventRecord(g.ffEv[2][q], sF));
+                CK(cudaStreamWaitEvent(sB, g.ffEv[2][q], 0));
                 const int r0 = ownedEnd(cNext), r1 = ownedEnd(cEnd);
                 if (rans) {
                     dim3 tr(32, 4, 1);
                     dim3 gr((d.nx + 31) / 32, (d.ny + 3) / 4, r1 - r0);
                     KT_BEGIN(K_SA, sB);
-                    k_sa<<<gr, tr, 0, sB>>>(d, b.dev, 0, MffdEpi{nullptr, 0}, r0, 1 + r1);
+                    k_sa<<<gr, tr, 0, sB>>>(d, b.dev, MffdEpi{nullptr, 0}, r0, 1 + r1);
                     KT_END(K_SA, sB);
                 }
                 KT_BEGIN(K_RESID, sB);
-                const int rc = launch_flowres_tile(d, b.dev, g.prm, (int)((b.dev.p - b.dev.w) / d.N), 1.0, 1, true, 0, sB, MffdEpi{nullptr, 0}, kc,
-                                                   cNext, cEnd - cNext);
+                const int rc = launch_flowres_tile(d, b.dev, g.prm, g.env, (int)((b.dev.p - b.dev.w) / d.N), 1.0, 1, true, 0, sB, MffdEpi{nullptr, 0},
+                                                   kc, cNext, cEnd - cNext);
                 KT_END(K_RESID, sB);
                 if (rc) return fail("tile kernel launch failed inside the form-function pipeline");
                 const long long q0 = (long long)r0 * plane, q1 = (long long)r1 * plane;
                 KT_BEGIN(K_MFFD, sB);
                 k_nkvec<<<(unsigned)((q1 - q0 + 255) / 256), 256, 0, sB>>>(d, b.dev, b.nw, nullptr, nullptr, g.nkY + off, 1.0, 2, q0, q1);
                 KT_END(K_MFFD, sB);
-                CK(cudaEventRecord(g_ffEv[1][q], sB));
-                CK(cudaStreamWaitEvent(g_ffOut, g_ffEv[1][q], 0));
-                CK(cudaMemcpyAsync(rVec + off + q0, g.nkY + off + q0, (size_t)(q1 - q0) * sizeof(double), cudaMemcpyDeviceToHost, g_ffOut));
+                CK(cudaEventRecord(g.ffEv[1][q], sB));
+                CK(cudaStreamWaitEvent(g.ffOut, g.ffEv[1][q], 0));
+                CK(cudaMemcpyAsync(rVec + off + q0, g.nkY + off + q0, (size_t)(q1 - q0) * sizeof(double), cudaMemcpyDeviceToHost, g.ffOut));
                 cNext = cEnd;
             }
         }
         off += (long long)d.nz * plane;
     }
     // join: everything meets on the library stream again
-    CK(cudaEventRecord(g_ffEv[3][1], g_ffIn));
-    CK(cudaStreamWaitEvent(sF, g_ffEv[3][1], 0));
-    CK(cudaEventRecord(g_ffEv[3][2], g_ffOut));
-    CK(cudaStreamWaitEvent(sF, g_ffEv[3][2], 0));
-    if (twoStreams) {
-        CK(cudaEventRecord(g_ffEv[3][3], sB));
-        CK(cudaStreamWaitEvent(sF, g_ffEv[3][3], 0));
-    }
+    CK(cudaEventRecord(g.ffEv[3][1], g.ffIn));
+    CK(cudaStreamWaitEvent(sF, g.ffEv[3][1], 0));
+    CK(cudaEventRecord(g.ffEv[3][2], g.ffOut));
+    CK(cudaStreamWaitEvent(sF, g.ffEv[3][2], 0));
+    CK(cudaEventRecord(g.ffEv[3][3], sB));
+    CK(cudaStreamWaitEvent(sF, g.ffEv[3][3], 0));
     CK(cudaGetLastError());
     return 0;
 }
@@ -1325,19 +1283,9 @@ static int form_function_pipelined(const double* wVec, double* rVec, long long n
         if (!b.alive || b.level != 1) continue;
         if (!b.haveMetrics || b.nOrphans || !tile_kernel_applies(b.d, b.dev, residual_discr(1, true)) || b.d.nz < 16) return -1;
     }
-    if (!g_ffIn) {
-        CK(cudaStreamCreateWithFlags(&g_ffIn, cudaStreamNonBlocking));
-        CK(cudaStreamCreateWithFlags(&g_ffOut, cudaStreamNonBlocking));
-        CK(cudaStreamCreateWithFlags(&g_ffBack, cudaStreamNonBlocking));
-        for (int a = 0; a < 4; a++) for (int q = 0; q < 34; q++) CK(cudaEventCreateWithFlags(&g_ffEv[a][q], cudaEventDisableTiming));
-    }
-    set_l2_window();
-    int twoStreams = 1;
-    if (const char* e = getenv("ADFB_FF_STREAMS")) twoStreams = atoi(e) >= 2 ? 1 : 0;
-    // one graph per (wVec, rVec, slabs, streams): an NK solve calls with the same PETSc vectors over and over
+    // one graph per (wVec, rVec, slabs): an NK solve calls with the same PETSc vectors over and over
     unsigned long long h = 1469598103934665603ull;
-    for (unsigned long long v : {(unsigned long long)(uintptr_t)wVec, (unsigned long long)(uintptr_t)rVec, (unsigned long long)wantSlabs,
-                                 (unsigned long long)twoStreams})
+    for (unsigned long long v : {(unsigned long long)(uintptr_t)wVec, (unsigned long long)(uintptr_t)rVec, (unsigned long long)wantSlabs})
         h = (h ^ v) * 1099511628211ull;
     const unsigned long long key = (12ull << 40) | (h & 0xffffffffffull);
     {   // a handful of vector pairs at most: forget the oldest graph beyond that
@@ -1351,7 +1299,7 @@ static int form_function_pipelined(const double* wVec, double* rVec, long long n
             }
         }
     }
-    const int rc = run_graphed(key, [&]() { return form_function_pipe_body(wVec, rVec, wantSlabs, twoStreams); });
+    const int rc = run_graphed(key, [&]() { return form_function_pipe_body(wVec, rVec, wantSlabs); });
     if (rc) return rc;
     CK(cudaStreamSynchronize(g.stream));
     return 0;
@@ -1542,7 +1490,7 @@ int adfb_timestep(int level, int onlyRadii) {
         dim3 tb(32, 4, 2);
         dim3 gr((b.d.NI + 31) / 32, (b.d.NJ + 3) / 4, (b.d.NK + 1) / 2);
         KT_BEGIN(K_PREP, g.stream);
-        launch_pdl(k_prep, gr, tb, g.stream, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, 0, INT_MAX, residual_discr(level, false), scaleRad);
+        launch_pdl(k_prep, gr, tb, g.stream, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, INT_MAX, residual_discr(level, false), scaleRad);
         KT_END(K_PREP, g.stream);
     }
     CK(cudaGetLastError());
@@ -1560,7 +1508,7 @@ static int adfb_smoother_residual_body(int level, int rkStage) {
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         // coarse level: initRes starts from the residual forcing term (dw = wr)
-        if (launch_residual_core(b.d, b.dev, g.prm, residual_discr(level, false), ADFB_RES_FLOW, rFil, 1, 0, g.stream,
+        if (launch_residual_core(b.d, b.dev, g.prm, g.env, residual_discr(level, false), ADFB_RES_FLOW, rFil, 1, 0, g.stream,
                                  above_ground(level) ? g.mgInitWr : 0))
             return fail("residual launch failed");
         // the primitive <-> conservative round trip that inviscidDissFluxScalarCoarse leaves on w (the matrix form does not convert)
@@ -1573,7 +1521,6 @@ int adfb_smoother_residual(int level, int rkStage) {
     ADFB_RANGE("adfb_smoother_residual");
     NEED_INIT();
     const unsigned long long key = (3ull << 40) | ((unsigned long long)level << 32) | ((unsigned)g.mgInitWr << 8) | (unsigned)rkStage;
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_smoother_residual_body(level, rkStage); });
 }
 
@@ -1587,7 +1534,7 @@ static int adfb_rk_stage_body(int level, int rkStage) {
         // currentCfl = cflCoarse unless currentLevel == 1; second halos only on the ground level (smoothers.F90:131-140)
         AdfbParams prmL = g.prm;
         if (level > 1) prmL.cfl = g.prm.cflCoarse;
-        if (launch_rk_update(b.d, b.dev, prmL, rkStage, g.stream, above_ground(level) ? 5 : 0)) return fail("RK update launch failed");
+        if (launch_rk_update(b.d, b.dev, prmL, g.env, rkStage, g.stream, above_ground(level) ? 5 : 0)) return fail("RK update launch failed");
     }
     // whalo2(level, 1, nwf, T, T, T) / whalo1 on coarse levels (the pattern of the level holds the matching lists):
     // the trailing computeEtotBlock is idempotent here unless an overset pattern interpolates into fringe cells.
@@ -1606,7 +1553,6 @@ int adfb_rk_stage(int level, int rkStage) {
     ADFB_RANGE("adfb_rk_stage");
     NEED_INIT();
     const unsigned long long key = (2ull << 40) | ((unsigned long long)level << 32) | (unsigned)rkStage;
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_rk_stage_body(level, rkStage); });
 }
 
@@ -1619,7 +1565,7 @@ static int adfb_dadi_step_body(int level) {
         AdfbParams prmL = g.prm;   // coarse levels: cflCoarse, first halos only, frozen eddy viscosity (smoothers.F90:463-472)
         if (level > 1) prmL.cfl = g.prm.cflCoarse;
         if (launch_dadi(b.d, b.dev, prmL, g.stream)) return fail("DADI launch failed");
-        if (launch_dadi_update(b.d, b.dev, prmL, g.stream, above_ground(level) ? 5 : 0)) return fail("DADI update launch failed");
+        if (launch_dadi_update(b.d, b.dev, prmL, g.env, g.stream, above_ground(level) ? 5 : 0)) return fail("DADI update launch failed");
         if (launch_bc_levels(b.d, b.dev, b.subfaces, above_ground(level) ? 0 : 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (halo_exchange_impl(level, 1, 5, 1, 1, overset_present(level))) return 1;
@@ -1630,7 +1576,6 @@ int adfb_dadi_step(int level) {
     ADFB_RANGE("adfb_dadi_step");
     NEED_INIT();
     const unsigned long long key = (4ull << 40) | ((unsigned long long)level << 32);
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_dadi_step_body(level); });
 }
 
@@ -1648,7 +1593,6 @@ int adfb_dadi_cycle(int level, int nSubiterations) {
     ADFB_RANGE("adfb_dadi_cycle");
     NEED_INIT();
     const unsigned long long key = (7ull << 40) | ((unsigned long long)level << 32) | (unsigned)nSubiterations;
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_dadi_cycle_body(level, nSubiterations); });
 }
 
@@ -1673,7 +1617,6 @@ int adfb_sa_ddadi(int level, int nSubIterTurb) {
     ADFB_RANGE("adfb_sa_ddadi");
     NEED_INIT();
     const unsigned long long key = (5ull << 40) | ((unsigned long long)level << 32) | (unsigned)nSubIterTurb;
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_sa_ddadi_body(level, nSubIterTurb); });
 }
 
@@ -1696,7 +1639,6 @@ int adfb_rk_cycle(int level) {
     ADFB_RANGE("adfb_rk_cycle");
     NEED_INIT();
     const unsigned long long key = (6ull << 40) | ((unsigned long long)level << 32);
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_rk_cycle_body(level); });
 }
 
@@ -2134,7 +2076,6 @@ int adfb_mg_restrict(int fineLevel) {
     NEED_INIT();
     if (!g.havePrm) return fail("adfb_mg_restrict: adfb_set_params has not been called");
     const unsigned long long key = (8ull << 40) | ((unsigned long long)fineLevel << 32);
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_mg_restrict_body(fineLevel); });
 }
 
@@ -2172,7 +2113,6 @@ int adfb_mg_prolong(int fineLevel) {
     NEED_INIT();
     if (!g.havePrm) return fail("adfb_mg_prolong: adfb_set_params has not been called");
     const unsigned long long key = (9ull << 40) | ((unsigned long long)fineLevel << 32);
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_mg_prolong_body(fineLevel); });
 }
 
@@ -2252,7 +2192,6 @@ int adfb_mg_prolong_solution(int fineLevel) {
     if (fineLevel < 1 || g.groundLevel != fineLevel + 1)
         return fail("adfb_mg_prolong_solution: the ground level must be %d (adfb_set_ground_level), it is %d", fineLevel + 1, g.groundLevel);
     const unsigned long long key = (11ull << 40) | ((unsigned long long)fineLevel << 32);
-    set_l2_window();
     return run_graphed(key, [&]() { return adfb_mg_prolong_solution_body(fineLevel); });
 }
 
@@ -2300,7 +2239,6 @@ int adfb_mg_cycle(int nSteps, const int* cycling, int smoother) {
     for (int n = 0; n < nSteps; n++) h = (h ^ (unsigned long long)(cycling[n] + 2)) * 1099511628211ull;
     h = (h ^ (unsigned long long)(smoother + 7)) * 1099511628211ull;
     const unsigned long long key = (10ull << 40) | (h & 0xffffffffffull);
-    set_l2_window();
     std::vector<int> cyc(cycling, cycling + nSteps);
     return run_graphed(key, [&]() { return adfb_mg_cycle_body(nSteps, cyc.data(), smoother); });
 }

@@ -311,6 +311,7 @@ struct DtSmem {
     double in[2][4][32][ADFB_DT_CH + 1];   // [stage][array][line][cell]; odd pitch: conflict-free 64-bit accesses down a column
     double out[2][32][ADFB_DT_CH + 1];
 };
+static const size_t kDadiTileSmem = sizeof(DtSmem) * ADFB_DT_WARPS;   // dynamic shared memory of one CTA
 __device__ __forceinline__ void dt_cp8(double* dst, const double* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
@@ -468,13 +469,10 @@ static int launch_dadi(const Dims& d, const BlockDev& b, const AdfbParams& prm, 
     // i lines (sd == 1) take the tiled walk: in the per-thread walk neighbouring threads own lines a whole row apart
     auto thomas = [&](int sd, int nl, int s1, int n1, int s2, int n2) {
         if (sd == 1) {
-            static bool once = false;
-            const size_t smem = sizeof(DtSmem) * ADFB_DT_WARPS;
-            if (!once) { cudaFuncSetAttribute(k_dadi_thomas_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); once = true; }
             const long long items = (long long)((n1 + 31) / 32) * n2 * 5;
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((unsigned)((items + ADFB_DT_WARPS - 1) / ADFB_DT_WARPS)); cfg.blockDim = dim3(32 * ADFB_DT_WARPS);
-            cfg.dynamicSmemBytes = smem; cfg.stream = s;
+            cfg.dynamicSmemBytes = kDadiTileSmem; cfg.stream = s;
             cudaLaunchAttribute attr[1];
             attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
             attr[0].val.programmaticStreamSerializationAllowed = 1;

@@ -986,24 +986,16 @@ static int fused_mode() {   // ADFB_FUSED: 0 = off (k_nodal/k_faces/k_div), 1 = 
 
 // returns 0 on success, -1 when the tile kernel does not apply (caller uses the general kernels), > 0 on error
 // kChunkForce > 0: that many planes per CTA instead of the wave-fitted chunk; zOff / zCount: only the k chunks zOff .. zOff+zCount-1
-static int launch_flowres_tile(const Dims& d, const BlockDev& b, const AdfbParams& prm, int nw, double rFil, int doDiss, bool merged,
-                               int persistFw, cudaStream_t stream, MffdEpi mf = MffdEpi{nullptr, 0}, int kChunkForce = 0, int zOff = 0,
-                               int zCount = -1) {
-    static int nSM = 0;
-    static size_t smemMax = 0;
-    if (!nSM) {
-        int dev = 0, v = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&nSM, cudaDevAttrMultiProcessorCount, dev);
-        cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-        smemMax = (size_t)v;
-    }
+// (adfb_init raises the dynamic shared memory limit of every k_flowres instance to env.smemOptin)
+static int launch_flowres_tile(const Dims& d, const BlockDev& b, const AdfbParams& prm, const LaunchEnv& env, int nw, double rFil, int doDiss,
+                               bool merged, int persistFw, cudaStream_t stream, MffdEpi mf = MffdEpi{nullptr, 0}, int kChunkForce = 0,
+                               int zOff = 0, int zCount = -1) {
     const bool viscous = prm.equations != ADFB_EULER;
     bool tma = fused_mode() >= 2 && !(d.NI & 1);
-    FTile t = ftile_choose(d, tma, nSM);
+    FTile t = ftile_choose(d, tma, env.nSM);
     if (kChunkForce > 0) t.kChunk = kChunkForce;
     if (!merged) t.smemBytes += (size_t)(FT_NFLUX_SPLIT - FT_NFLUX) * FT_S0 * sizeof(double);   // central and dissipative fluxes exchanged apart
-    if (!ftile_fits(t) || t.smemBytes > smemMax) return -1;
+    if (!ftile_fits(t) || t.smemBytes > env.smemOptin) return -1;
     FTmaMaps maps;
     memset(&maps, 0, sizeof maps);
     if (tma) {
@@ -1022,12 +1014,7 @@ static int launch_flowres_tile(const Dims& d, const BlockDev& b, const AdfbParam
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     cudaError_t e;
-#define FT_LAUNCH(V, M)                                                                                                         \
-    do {                                                                                                                        \
-        static bool attrSet = false;                                                                                            \
-        if (!attrSet) { cudaFuncSetAttribute(k_flowres<V, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemMax); attrSet = true; } \
-        e = cudaLaunchKernelEx(&cfg, k_flowres<V, M>, d, b, t, rFil, doDiss, persistFw, nw, mf, maps, zOff);                               \
-    } while (0)
+#define FT_LAUNCH(V, M) e = cudaLaunchKernelEx(&cfg, k_flowres<V, M>, d, b, t, rFil, doDiss, persistFw, nw, mf, maps, zOff)
     if (viscous) { if (merged) FT_LAUNCH(true, true); else FT_LAUNCH(true, false); }
     else { if (merged) FT_LAUNCH(false, true); else FT_LAUNCH(false, false); }
 #undef FT_LAUNCH

@@ -49,13 +49,6 @@
 #ifndef NODAL_MINB
 #define NODAL_MINB 1
 #endif
-static inline dim3 tune_block(const char* env, dim3 dflt) {
-    const char* e = getenv(env);
-    if (!e) return dflt;
-    int x = 0, y = 0, z = 0;
-    if (sscanf(e, "%d,%d,%d", &x, &y, &z) == 3 && x > 0 && y > 0 && z > 0) return dim3(x, y, z);
-    return dflt;
-}
 
 #define IRHO 0
 #define IVX 1
@@ -75,22 +68,15 @@ __global__ void __launch_bounds__(256) k_geom(Dims d, BlockDev b) {
 // ---------------------------------------------------------------------------
 // k_prep: entropy (inviscidDissFluxScalar, blockette.F90:3055-3089), speed of sound squared
 // (:5168-5203), spectral radii and local time step (timeStep, :1899-2148).
-// part: 0 = every box cell, 1 = owned cells without a halo neighbour (3:nx, ...: the pressure switch of dtl reads the six
-// neighbours), 2 = the rest (the first part does not need the BCs and runs beside them, see residual_body)
 // kOff / kTop: the planes kOff .. kTop only (slab pipeline of adfb_form_function); 0 / INT_MAX: all of them
 // disc: the discretisation of the residual that reads ss (residual_discr); scaleRad: directional scaling of the radii
 // (doScaling of timeStep: always on the blockette path, dirScaling .and. currentLevel <= groundLevel on the block path)
-__global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, int doRad, int part, int kOff, int kTop, int disc,
-                                              int scaleRad) {
+__global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, int doRad, int kOff, int kTop, int disc, int scaleRad) {
     ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_pdl)
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int j = blockIdx.y * blockDim.y + threadIdx.y;
     const int k = blockIdx.z * blockDim.z + threadIdx.z + kOff;
     if (i > d.ib || j > d.jb || k > d.kb || k > kTop) return;
-    if (part) {
-        const bool inner = i >= 3 && i < d.il && j >= 3 && j < d.jl && k >= 3 && k < d.kl;
-        if (inner != (part == 1)) return;
-    }
     const int N = (int)d.N, sJ = (int)d.sJ, sK = (int)d.sK;
     const int c = i + sJ * j + sK * k;
     const double gam = c_prm.gammaInf;
@@ -742,18 +728,12 @@ __device__ __forceinline__ double sa_source(const BlockDev& b, int N, int sJ, in
 
 // k_sa: SA row of one owned cell: source, advection k/j/i, diffusion k/j/i, scaling
 // (blockette.F90:623-627, :1872-1897)
-// part: 0 = every owned cell, 1 = cells at least two layers away from the block boundary (their stencil holds no halo
-// cell: they do not need the BCs / the exchange), 2 = the boundary shell
 // kOff / kTop: the owned planes 2 + kOff .. kTop only (slab pipeline); 0 / INT_MAX: all of them
-__global__ void __launch_bounds__(SA_TPB, SA_MINB) k_sa(Dims d, BlockDev b, int part, MffdEpi mf, int kOff, int kTop) {
+__global__ void __launch_bounds__(SA_TPB, SA_MINB) k_sa(Dims d, BlockDev b, MffdEpi mf, int kOff, int kTop) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x + 2;
     const int j = blockIdx.y * blockDim.y + threadIdx.y + 2;
     const int k = blockIdx.z * blockDim.z + threadIdx.z + 2 + kOff;
     if (i > d.il || j > d.jl || k > d.kl || k > kTop) return;
-    if (part) {
-        const bool inner = i >= 4 && i <= d.il - 2 && j >= 4 && j <= d.jl - 2 && k >= 4 && k <= d.kl - 2;
-        if (inner != (part == 1)) return;
-    }
     const int N = (int)d.N, sJ = (int)d.sJ, sK = (int)d.sK;
     const int c = i + sJ * j + sK * k;
     const double rblank = dmax_((double)b.iblank[c], 0.0);
@@ -859,12 +839,10 @@ static bool split_faces() {
 static bool tile_kernel_applies(const Dims& d, const BlockDev& b, int disc) {
     return fused_mode() > 0 && !b.coarse && disc == ADFB_DISS_SCALAR && !split_faces();
 }
-enum { RC_PREP_OWNED = 1, RC_PREP_HALO = 2, RC_SA_INNER = 4, RC_SA_SHELL = 8, RC_FLOW = 16, RC_ALL = 31 };
 // disc: the discretisation of this residual (residual_discr in adflow_b200.cu); on a level above the ground level it is
 // spaceDiscrCoarse and selects the first-order coarse-level fluxes
-static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbParams& prm, int disc, unsigned flags, double rFil,
-                                int persistFw, int doRad, cudaStream_t stream, int initWr = 0, int parts = RC_ALL,
-                                MffdEpi mf = MffdEpi{nullptr, 0}) {
+static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbParams& prm, const LaunchEnv& env, int disc, unsigned flags,
+                                double rFil, int persistFw, int doRad, cudaStream_t stream, int initWr = 0, MffdEpi mf = MffdEpi{nullptr, 0}) {
     const int flowRes = (flags & ADFB_RES_FLOW) != 0;
     const int turbRes = ((flags & ADFB_RES_TURB) != 0) && prm.equations == ADFB_RANS;
     const int updateDt = 1;  // blockette timeStep always computes dtl (blockette.F90:1929-1932)
@@ -881,48 +859,34 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     // The SA row reads only the state and static geometry and writes dw(itu1); the flow rows write dw(1:5).
     // The two chains are independent, so k_sa is forked onto a side stream (also inside graph capture) and
     // joined at the end: both chains are latency bound, their warps interleave on the SMs.
-    static cudaStream_t s_side = nullptr;
-    static cudaEvent_t s_fork = nullptr, s_join = nullptr;
     static int s_conc = -1;
     if (s_conc < 0) {
         const char* e = getenv("ADFB_SA_CONCURRENT");
         s_conc = e ? atoi(e) : 1;
     }
-    const int saPart = ((parts & RC_SA_INNER) && (parts & RC_SA_SHELL)) ? 0 : (parts & RC_SA_INNER) ? 1 : 2;
-    const bool fork = turbRes && flowRes && s_conc && !g_kt.on && (parts & RC_FLOW);
-    if (turbRes && (parts & (RC_SA_INNER | RC_SA_SHELL))) {
-        dim3 tr = tune_block("ADFB_SA_BLOCK", dim3(32, 4, 1));
+    const bool fork = turbRes && flowRes && s_conc && !g_kt.on;
+    if (turbRes) {
+        dim3 tr(32, 4, 1);
         dim3 g((d.nx + tr.x - 1) / tr.x, (d.ny + tr.y - 1) / tr.y, (d.nz + tr.z - 1) / tr.z);
         if (fork) {
-            if (!s_side) {
-                // lowest priority: the SA row fills the issue slots the tile kernel leaves, it must not take SMs from it
-                int prLo = 0, prHi = 0;
-                cudaDeviceGetStreamPriorityRange(&prLo, &prHi);
-                if (cudaStreamCreateWithPriority(&s_side, cudaStreamNonBlocking, prLo) != cudaSuccess) return 1;
-                if (cudaEventCreateWithFlags(&s_fork, cudaEventDisableTiming) != cudaSuccess) return 1;
-                if (cudaEventCreateWithFlags(&s_join, cudaEventDisableTiming) != cudaSuccess) return 1;
-            }
-            cudaStreamCopyAttributes(s_side, stream);   // same L2 access-policy window as the main stream
-            cudaEventRecord(s_fork, stream);
-            cudaStreamWaitEvent(s_side, s_fork, 0);
-            k_sa<<<g, tr, 0, s_side>>>(d, b, saPart, mf, 0, INT_MAX);
+            cudaEventRecord(env.saFork, stream);
+            cudaStreamWaitEvent(env.saStream, env.saFork, 0);
+            k_sa<<<g, tr, 0, env.saStream>>>(d, b, mf, 0, INT_MAX);
             g_kt.launches++; g_kt.count[K_SA]++;
-            cudaEventRecord(s_join, s_side);
+            cudaEventRecord(env.saJoin, env.saStream);
         } else {
             KT_BEGIN(K_SA, stream);
-            k_sa<<<g, tr, 0, stream>>>(d, b, saPart, mf, 0, INT_MAX);
+            k_sa<<<g, tr, 0, stream>>>(d, b, mf, 0, INT_MAX);
             KT_END(K_SA, stream);
         }
     }
-    if ((doRad || (flowRes && doDiss)) && (parts & (RC_PREP_OWNED | RC_PREP_HALO))) {
-        const int prepPart = ((parts & RC_PREP_OWNED) && (parts & RC_PREP_HALO)) ? 0 : (parts & RC_PREP_OWNED) ? 1 : 2;
+    if (doRad || (flowRes && doDiss)) {
         dim3 g((d.NI + tb.x - 1) / tb.x, (d.NJ + tb.y - 1) / tb.y, (d.NK + tb.z - 1) / tb.z);
         KT_BEGIN(K_PREP, stream);
-        launch_pdl(k_prep, g, tb, stream, d, b, updateDt, doRad, prepPart, 0, INT_MAX, disc, (int)!b.coarse);
+        launch_pdl(k_prep, g, tb, stream, d, b, updateDt, doRad, 0, INT_MAX, disc, (int)!b.coarse);
         KT_END(K_PREP, stream);
     }
     // tile kernel (fused_kernels.cuh): exact central + scalar-JST (+ viscous) flow rows in one launch
-    if (!(parts & RC_FLOW)) return (int)cudaGetLastError();
     bool fusedDone = false;
     // (smoother path, persistFw: the tile kernel exchanges central and dissipative fluxes separately with two more CTA
     // barriers per plane and was slower than k_nodal/k_faces/k_div there; ADFB_FUSED_SMOOTHER=1 selects it anyway)
@@ -933,14 +897,14 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     if (flowRes && fused_mode() > 0 && (!persistFw || fusedSmoother == 1 || (fusedSmoother == 2 && doDiss)) && !b.coarse && disc == ADFB_DISS_SCALAR && !dissApprox && !viscApprox && !initWr &&
         !(flags & ADFB_RES_STORE_WALL) && !split_faces()) {
         KT_BEGIN(K_RESID, stream);
-        const int rc = launch_flowres_tile(d, b, prm, (int)((b.p - b.w) / d.N), rFil, doDiss, !persistFw, persistFw, stream, mf);
+        const int rc = launch_flowres_tile(d, b, prm, env, (int)((b.p - b.w) / d.N), rFil, doDiss, !persistFw, persistFw, stream, mf);
         KT_END(K_RESID, stream);
         if (rc > 0) return 1;
         fusedDone = rc == 0;
     }
     if (mf.rec && flowRes && !fusedDone) return 1;   // the fused matrix-free epilogue lives in the tile kernel
     if (flowRes && doDiss && !fusedDone) {
-        dim3 tn = tune_block("ADFB_NODAL_BLOCK", dim3(32, 4, 2));
+        dim3 tn(32, 4, 2);
         dim3 g((d.ie + tn.x - 1) / tn.x, (d.je + tn.y - 1) / tn.y, (d.ke + tn.z - 1) / tn.z);
         KT_BEGIN(K_NODAL, stream);
         if (gradAos) launch_pdl(k_nodal<true>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
@@ -948,7 +912,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         KT_END(K_NODAL, stream);
     }
     if (flowRes && !fusedDone) {
-        dim3 tr = tune_block("ADFB_FACES_BLOCK", dim3(32, 4, 1));
+        dim3 tr(32, 4, 1);
         dim3 g((d.il + tr.x - 1) / tr.x, (d.jl + tr.y - 1) / tr.y, (d.kl + tr.z - 1) / tr.z);
         const bool merged = !persistFw;
         KT_BEGIN(K_RESID, stream);
@@ -1012,6 +976,6 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         else launch_pdl(k_div<false>, g2, tb, stream, d, b, rFil, persistFw, initWr);
         KT_END(K_DIV, stream);
     }
-    if (fork) cudaStreamWaitEvent(stream, s_join, 0);
+    if (fork) cudaStreamWaitEvent(stream, env.saJoin, 0);
     return (int)cudaGetLastError();
 }

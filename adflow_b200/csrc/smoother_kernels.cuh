@@ -538,6 +538,7 @@ __global__ void __launch_bounds__(64) k_resavg_sweep(Dims d, BlockDev b, int dir
 // HBM traffic 88 B per cell and direction (epz + dw in, dw out) instead of 192 B with the forward-swept values in
 // global memory, and the serial walks never wait for HBM.  Same operations on the same operands as k_resavg_sweep.
 #define ADFB_RA_THREADS 768   // copy phases: enough loads in flight to fill the SM's share of HBM bandwidth
+static const size_t kResavgSmemMax = 220 * 1024;   // dynamic shared memory a CTA may take
 // lines are numbered id = (q1 - 2) + n1 (q2 - 2); a CTA takes LPC consecutive ids (LPC is sized on the host so that the
 // grid is one wave of the SMs), LP = padded pitch of the shared arrays (odd: conflict free along and across the lines)
 __global__ void __launch_bounds__(ADFB_RA_THREADS) k_resavg_lines(Dims d, BlockDev b, int dir, long long sd, int n, long long s1, int n1,
@@ -613,9 +614,7 @@ __global__ void __launch_bounds__(ADFB_RA_THREADS) k_resavg_lines(Dims d, BlockD
 
 // lines per CTA of the shared-memory line kernels: one wave of one CTA per SM if the lines fit, else the largest count
 // that fits (nArr arrays of n x LP doubles + the line table)
-static int lines_per_cta(long long nLinesTotal, int n, int nArr, int maxLpc, size_t lim, int* LPout, size_t* bytesOut) {
-    static int nSM = 0;
-    if (!nSM) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nSM, cudaDevAttrMultiProcessorCount, dev); }
+static int lines_per_cta(long long nLinesTotal, int n, int nArr, int maxLpc, size_t lim, int nSM, int* LPout, size_t* bytesOut) {
     auto bytes = [&](int lpc) { const int LP = lpc | 1; return (size_t)nArr * n * LP * sizeof(double) + (size_t)lpc * sizeof(long long); };
     int lpc = (int)((nLinesTotal + nSM - 1) / nSM);
     if (lpc < 4) lpc = (int)(nLinesTotal < 4 ? nLinesTotal : 4);
@@ -781,7 +780,7 @@ static BcList make_bc_list(const Dims& d, const std::vector<AdfbSubface>& subs, 
     return L;
 }
 
-static int launch_residual_averaging(const Dims& d, const BlockDev& b, const AdfbParams& prm, cudaStream_t s) {
+static int launch_residual_averaging(const Dims& d, const BlockDev& b, const AdfbParams& prm, const LaunchEnv& env, cudaStream_t s) {
     const double rfl0 = 0.5 * prm.cfl / prm.cflLimit;
     {
         dim3 tb(32, 4, 2);
@@ -797,9 +796,8 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
     auto run = [&](int dir, long long sd, int n, long long s1, int n1, long long s2, int n2) {
         if (n <= 1) return;
         KT_BEGIN(K_RK, s);
-        const size_t lim = 220 * 1024;
         int LP = 0; size_t smem = 0;
-        const int lpc = lines_per_cta((long long)n1 * n2, n, 8, ADFB_RA_THREADS / 5, lim, &LP, &smem);
+        const int lpc = lines_per_cta((long long)n1 * n2, n, 8, ADFB_RA_THREADS / 5, kResavgSmemMax, env.nSM, &LP, &smem);
         if (lpc) {
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((unsigned)(((long long)n1 * n2 + lpc - 1) / lpc)); cfg.blockDim = dim3(ADFB_RA_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
@@ -807,8 +805,6 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
             attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
             attr[0].val.programmaticStreamSerializationAllowed = 1;
             cfg.attrs = attr; cfg.numAttrs = 1;
-            static bool once = false;
-            if (!once) { cudaFuncSetAttribute(k_resavg_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lim); once = true; }
             cudaLaunchKernelEx(&cfg, k_resavg_lines, d, b, dir, sd, n, s1, n1, s2, n2, lpc, LP);
         } else {   // not even one line fits into shared memory (n >= 3520 cells)
             launch_pdl(k_resavg_sweep, dim3((n1 + 31) / 32, (n2 + 1) / 2, 5), tb, s, d, b, dir, sd, n, s1, n1, s2, n2);
@@ -821,7 +817,8 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
     return (int)cudaGetLastError();
 }
 
-static int launch_rk_update(const Dims& d, const BlockDev& b, const AdfbParams& prm, int rkStage, cudaStream_t s, int nwOverride = 0) {
+static int launch_rk_update(const Dims& d, const BlockDev& b, const AdfbParams& prm, const LaunchEnv& env, int rkStage, cudaStream_t s,
+                            int nwOverride = 0) {
     const double tmp = prm.cfl * prm.etaRK[rkStage - 1];
     const bool smooth = prm.resAveraging == 1 || (prm.resAveraging == 2 && (rkStage % 2) == 1);
     dim3 tb(32, 4, 2);
@@ -831,7 +828,7 @@ static int launch_rk_update(const Dims& d, const BlockDev& b, const AdfbParams& 
         KT_BEGIN(K_RK, s);
         launch_pdl(k_rk_scale, g, tb, s, d, b, tmp);
         KT_END(K_RK, s);
-        if (launch_residual_averaging(d, b, prm, s)) return 1;
+        if (launch_residual_averaging(d, b, prm, env, s)) return 1;
         KT_BEGIN(K_RK, s);
         launch_pdl(k_rk_update, g, tb, s, d, b, 0, tmp, nw, 0);
         KT_END(K_RK, s);
@@ -844,9 +841,9 @@ static int launch_rk_update(const Dims& d, const BlockDev& b, const AdfbParams& 
 }
 
 // state update of executeDADIStep (smoothers.F90:595-650) after computedwDADI
-static int launch_dadi_update(const Dims& d, const BlockDev& b, const AdfbParams& prm, cudaStream_t s, int nwOverride = 0) {
+static int launch_dadi_update(const Dims& d, const BlockDev& b, const AdfbParams& prm, const LaunchEnv& env, cudaStream_t s, int nwOverride = 0) {
     if (prm.resAveraging == 1)  // rkStage == 0 in the DADI smoother: `alternate` never smooths (smoothers.F90:461-469)
-        if (launch_residual_averaging(d, b, prm, s)) return 1;
+        if (launch_residual_averaging(d, b, prm, env, s)) return 1;
     dim3 tb(32, 4, 2);
     dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, (d.nz + 1) / 2);
     KT_BEGIN(K_RK, s);
