@@ -15,6 +15,10 @@ only.  ``regime_case`` builds blocks that reach the other side:
   floors                              one plane whose internal energy lies below the pressure floor 1e-4 pInfCorr and
                                       nuTilde below the setW clip 1e-6 nuInf in the cells of another plane
   low_mach                            M 0.3, alpha 25 deg, far field on both j faces: far-field inflow and outflow on j
+  low_reynolds                        the default state with a free-stream pressure of 2 Pa instead of 20 kPa: a
+                                      Reynolds number of about 520 per unit block length instead of 5e6, so that the
+                                      viscous flux, the heat flux and the SA source terms are a sizeable part of the rows
+                                      they enter (tests/test_low_reynolds_terms.py measures each share)
 
 A contact that spans the block (contact_i/j/k) puts the low-density side against the far-field faces; an explicit
 smoother cycle on it diverges within one cycle in the reference's own executeRKStage as much as in the oracle (the two
@@ -31,8 +35,11 @@ from adflow_b200 import make_params
 from adflow_b200 import synthetic as syn
 from adflow_b200.params import EULER, RANS
 
-REGIMES = ("contact_i", "contact_j", "contact_k", "contact_pocket", "supersonic", "stagnation", "floors", "low_mach")
+REGIMES = ("contact_i", "contact_j", "contact_k", "contact_pocket", "supersonic", "stagnation", "floors", "low_mach",
+           "low_reynolds")
 FREE_STREAM = {"supersonic": (2.0, 20.0), "low_mach": (0.3, 25.0)}   # (Mach, alpha in degrees); M 0.8 / 1.8 deg otherwise
+PRESSURE = {"low_reynolds": 2.0}   # free-stream pressure in Pa; 20 kPa (make_params' default) otherwise
+LOW_CELL_RE = 1000.0               # cell Reynolds number below which a cell counts as viscous-dominated
 LOW_MACH_FACES = {syn.IMIN: syn.BC_FARFIELD, syn.IMAX: syn.BC_FARFIELD, syn.JMIN: syn.BC_FARFIELD,
                   syn.JMAX: syn.BC_FARFIELD, syn.KMIN: syn.BC_WALL, syn.KMAX: syn.BC_FARFIELD}
 DENSITY_JUMP = 1.0 / 8.0
@@ -62,14 +69,17 @@ def contact_plane(name, shape):
     return 2 + shape[a] // 2
 
 
-def regime_case(name, shape, options=None, at=None, seed=314):
+def regime_case(name, shape, options=None, at=None, seed=314, physical_faces=None):
     """(prm, hb) of regime `name` on a block of `shape` owned cells.  `at`: for the contact regimes, the first cell (box
-    index, owned cells are 2..n+1) of the low-density side; the jump lies on the face between at-1 and at."""
+    index, owned cells are 2..n+1) of the low-density side; the jump lies on the face between at-1 and at.
+    `physical_faces`: a face -> bcType layout in place of the regime's own."""
     if name not in REGIMES:
         raise KeyError(name)
     mach, alpha = FREE_STREAM.get(name, (0.8, 1.8))
-    prm = make_params(options, mach=mach, alpha_deg=alpha)
-    kw = {"physical_faces": LOW_MACH_FACES} if name == "low_mach" else {}
+    prm = make_params(options, mach=mach, alpha_deg=alpha, **({"P": PRESSURE[name]} if name in PRESSURE else {}))
+    if physical_faces is None and name == "low_mach":
+        physical_faces = LOW_MACH_FACES
+    kw = {} if physical_faces is None else {"physical_faces": physical_faces}
     hb = syn.make_block(*shape, prm, seed=seed, **kw)
     d, w = hb.d, hb.w
     p = hb.p.copy()
@@ -221,6 +231,24 @@ def sa_rr_unclipped(prm, hb):
     return nt * k2i * d2i / sst
 
 
+def cell_reynolds(prm, hb):
+    """rho |uInf| h / (rlv + rev) at the owned cells, h the largest of the cell's three widths vol / |s| (s averaged
+    over the two faces of a direction): where it is small the viscous flux is a sizeable part of the momentum rows.
+    The free-stream speed, not the local one, so that the cells next to a wall, where the synthetic velocity profile
+    goes to zero, do not count as viscous-dominated at every Reynolds number."""
+    d = hb.d
+    ow = d.owned()
+    I, J, K = ow
+    Im, Jm, Km = (slice(s.start - 1, s.stop - 1) for s in ow)
+    area = lambda s: np.linalg.norm(s, axis=-1)   # noqa: E731
+    widths = [hb.vol[ow] / (0.5 * (area(hb.si[I, J, K]) + area(hb.si[Im, J, K]))),
+              hb.vol[ow] / (0.5 * (area(hb.sj[I, J, K]) + area(hb.sj[I, Jm, K]))),
+              hb.vol[ow] / (0.5 * (area(hb.sk[I, J, K]) + area(hb.sk[I, J, Km])))]
+    u_inf = math.sqrt(prm.wInf[1] ** 2 + prm.wInf[2] ** 2 + prm.wInf[3] ** 2) / prm.wInf[0]
+    mu = hb.rlv[ow] + (hb.rev[ow] if prm.equations == RANS else 0.0)
+    return hb.w[ow + (0,)] * u_inf * np.maximum(np.maximum(widths[0], widths[1]), widths[2]) / mu
+
+
 def reach(prm, hb, regime=None):
     """branch counts of the input state (numpy only; `regime` is informational)"""
     d = hb.d
@@ -241,6 +269,8 @@ def reach(prm, hb, regime=None):
     v2 = (w[..., 1:4] ** 2).sum(-1)
     pe = (gam - 1.0) * (w[..., 4] - 0.5 * w[..., 0] * v2)
     r["p_floor"] = int((pe < PRESSURE_FLOOR * prm.pInfCorr).sum())
+    if prm.equations != EULER:
+        r["low_cell_re"] = int((cell_reynolds(prm, hb) < LOW_CELL_RE).sum())
     if hb.nw > 5:
         r["turb_clip"] = int((w[..., 5] < TURB_CLIP * prm.wInf[5]).sum())
         r["sa_rr_clip"] = int((sa_rr_unclipped(prm, hb) > 10.0).sum())

@@ -141,7 +141,7 @@ def _regime_rows_close(hb, regime, at, got, want, tol=1e-12):
     import regimes as R
 
     ow = hb.d.owned()
-    far = None if regime == "supersonic" else R.owned_away_from(hb, regime, at)
+    far = R.owned_away_from(hb, regime, at) if regime.startswith("contact") else None
     for l in range(5):
         a, b = got[ow + (l,)], want[ow + (l,)]
         assert np.isfinite(a).all(), l
@@ -150,7 +150,16 @@ def _regime_rows_close(hb, regime, at, got, want, tol=1e-12):
             assert rel_l2(a[far], b[far]) < tol, ("away from the jump", l, rel_l2(a[far], b[far]))
 
 
-REGIME_CASES = [(r, at) for r in ("contact_i", "contact_j", "contact_k") for at in SEAMS[r]] + [("supersonic", None)]
+# low_reynolds: the viscous flux, which the nodal gradients feed and nothing else, is 2e-2 .. 1 of the momentum and
+# energy rows (tests/test_low_reynolds_terms.py), so a gradient wrong at a tile or chunk seam cannot hide in the row.
+REGIME_CASES = [(r, at) for r in ("contact_i", "contact_j", "contact_k") for at in SEAMS[r]] + [("supersonic", None),
+                                                                                               ("low_reynolds", None)]
+
+
+def _reach_keys(regime):
+    if regime == "low_reynolds":
+        return ["low_cell_re"]
+    return ["sensor_cap_" + a for a in ("ijk" if regime == "supersonic" else regime[-1])]
 
 
 @pytest.mark.parametrize("regime,at", REGIME_CASES)
@@ -159,7 +168,7 @@ def test_emulated_tile_kernel_in_regimes(regime, at):
     from test_regimes_reach import assert_reaches
 
     prm, hb = R.regime_case(regime, (12, 10, 8), at=at)
-    assert_reaches(prm, hb, regime, ["sensor_cap_" + a for a in ("ijk" if regime == "supersonic" else regime[-1])])
+    assert_reaches(prm, hb, regime, _reach_keys(regime))
     ho = oracle_residual(prm, hb, FLOW | TURB)
     dw, _ = run_emul(prm, hb, ho, *TILE)
     _regime_rows_close(hb, regime, at, dw, ho.dw)
@@ -172,6 +181,10 @@ def test_emulated_smoother_path_in_regimes(regime, at):
     from oracle.pyoracle import Oracle
 
     prm, hb = R.regime_case(regime, (12, 10, 8), at=at)
+    if regime == "low_reynolds":
+        from test_regimes_reach import assert_reaches
+
+        assert_reaches(prm, hb, regime)
     h2 = hb.copy()
     o = Oracle(h2, prm)
     o.time_step(True)

@@ -19,6 +19,7 @@ EXPECT = {
     "stagnation": ["stagnant_i", "stagnant_j", "stagnant_k", "sa_rr_clip"],
     "floors": ["p_floor", "turb_clip", "sensor_cap_i", "matrix_sensor_cap_i"],
     "low_mach": ["ff_sub_in", "ff_sub_out"],
+    "low_reynolds": ["low_cell_re"],
 }
 
 
@@ -41,6 +42,14 @@ def test_smooth_state_reaches_none_of_them():
     smooth = R.reach(*case(*SHAPE))
     for k in ("sensor_cap_i", "sensor_cap_j", "sensor_cap_k", "ff_sup_in", "ff_sup_out", "p_floor", "turb_clip", "sa_rr_clip"):
         assert smooth[k] == 0, k
+
+
+@pytest.mark.parametrize("eq", ["RANS", "laminar NS"])
+def test_low_reynolds_cells_only_at_low_pressure(eq):
+    """at 20 kPa no owned cell is viscous-dominated; at the low_reynolds regime's 2 Pa every one is"""
+    assert R.reach(*case(*SHAPE, {"equationType": eq}))["low_cell_re"] == 0
+    prm, hb = R.regime_case("low_reynolds", SHAPE, {"equationType": eq})
+    assert R.reach(prm, hb)["low_cell_re"] == hb.d.nx * hb.d.ny * hb.d.nz
 
 
 def test_low_mach_far_field_in_and_out_on_both_j_faces():
