@@ -160,14 +160,12 @@ struct KTimer {
 };
 static KTimer g_kt;
 
-// What the launch helpers need of the context: properties of the device it is bound to and the side stream of the SA row.
-// adfb_init reads and creates them for the device it binds, adfb_finalize releases them.
+// What the launch helpers need of the context: properties of the device it is bound to (adfb_init reads them for the
+// device it binds).
 struct LaunchEnv {
     int nSM = 0;                 // multiprocessors
     size_t smemOptin = 0;        // opt-in dynamic shared memory per CTA
-    // the SA row of the residual runs here beside the flow rows (launch_residual_core)
-    cudaStream_t saStream = nullptr;
-    cudaEvent_t saFork = nullptr, saJoin = nullptr;
+    int saCtasPerSM = 0;         // resident CTAs of the SA-row kernel k_sa per multiprocessor
 };
 
 // lanes per line for the partitioned Thomas kernels (tridiag_part.cuh): 8 lanes x <= 16 rows, 16 lanes x <= 16

@@ -296,24 +296,22 @@ void drop_graphs() {
 }
 
 // The streams, events and buffers of the context, for the device that is current.  The library stream carries the
-// latency-bound chains (BC levels, line solves) at the highest priority, and so does the stream of the SA row forked beside
-// the flow rows: that is the priority the SA row has run and been measured at (cudaStreamCopyAttributes from the library
-// stream, which carries the priority attribute, used to precede every fork).
+// latency-bound chains (BC levels, line solves) at the highest priority.
 int create_device_resources() {
     int prLo = 0, prHi = 0;
     CK(cudaDeviceGetStreamPriorityRange(&prLo, &prHi));
-    for (cudaStream_t* s : {&g.stream, &g.env.saStream}) CK(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, prHi));
+    CK(cudaStreamCreateWithPriority(&g.stream, cudaStreamNonBlocking, prHi));
     for (cudaStream_t* s : {&g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) CK(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
-    for (cudaEvent_t* e : {&g.env.saFork, &g.env.saJoin, &g.evPost, &g.evDone}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    for (cudaEvent_t* e : {&g.evPost, &g.evDone}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     for (auto& row : g.ffEv) for (cudaEvent_t& e : row) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     CK(cudaMalloc((void**)&g.dConst, 8 * sizeof(double)));
     CK(cudaMallocHost((void**)&g.hRed, 256 * sizeof(double)));
     return 0;
 }
 void release_device_resources() {
-    for (cudaEvent_t* e : {&g.env.saFork, &g.env.saJoin, &g.evPost, &g.evDone}) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
+    for (cudaEvent_t* e : {&g.evPost, &g.evDone}) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
     for (auto& row : g.ffEv) for (cudaEvent_t& e : row) { if (e) cudaEventDestroy(e); e = nullptr; }
-    for (cudaStream_t* s : {&g.stream, &g.env.saStream, &g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) { if (*s) cudaStreamDestroy(*s); *s = nullptr; }
+    for (cudaStream_t* s : {&g.stream, &g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) { if (*s) cudaStreamDestroy(*s); *s = nullptr; }
     if (g.dConst) cudaFree(g.dConst);
     g.dConst = nullptr;
     if (g.hRed) cudaFreeHost(g.hRed);
@@ -376,6 +374,8 @@ int adfb_init(int device, const void* ncclUniqueId, int rank, int nranks) {
             CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
         CK(cudaFuncSetAttribute(k_resavg_lines, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kResavgSmemMax));
         CK(cudaFuncSetAttribute(k_dadi_thomas_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDadiTileSmem));
+        CK(cudaFuncSetAttribute(k_sa, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_SMEM_BYTES));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g.env.saCtasPerSM, k_sa, SA_MAXT, SA_SMEM_BYTES));
     }
     g.device = device; g.rank = rank; g.nranks = nranks;
     g.err.clear();
@@ -1233,11 +1233,10 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
                 CK(cudaStreamWaitEvent(sB, g.ffEv[2][q], 0));
                 const int r0 = ownedEnd(cNext), r1 = ownedEnd(cEnd);
                 if (rans) {
-                    dim3 tr(32, 4, 1);
-                    dim3 gr((d.nx + 31) / 32, (d.ny + 3) / 4, r1 - r0);
                     KT_BEGIN(K_SA, sB);
-                    k_sa<<<gr, tr, 0, sB>>>(d, b.dev, MffdEpi{nullptr, 0}, r0, 1 + r1);
+                    const int rcSa = launch_sa(d, b.dev, g.env, MffdEpi{nullptr, 0}, r0, 1 + r1, sB);
                     KT_END(K_SA, sB);
+                    if (rcSa) return fail("SA row launch failed inside the form-function pipeline");
                 }
                 KT_BEGIN(K_RESID, sB);
                 const int rc = launch_flowres_tile(d, b.dev, g.prm, g.env, (int)((b.dev.p - b.dev.w) / d.N), 1.0, 1, true, 0, sB, MffdEpi{nullptr, 0},

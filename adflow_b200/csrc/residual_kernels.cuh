@@ -15,7 +15,8 @@
 //   k_prep   : box cells  -> ss (entropy), aa, radI/J/K, [dtl]
 //   k_nodal  : cells 1:ie -> dss(3); nodes 1:il -> 12 nodal gradients
 //   k_faces  : cells 1:il x 1:jl x 1:kl -> central - JST - viscous flux of the 3 plus faces
-//   k_div    : owned cells -> SA source/advection/diffusion row + flux divergence -> dw
+//   k_div    : owned cells -> flux divergence -> dw(1:5)
+//   k_sa     : owned cells -> SA source/advection/diffusion row -> dw(itu1) (sa_tile.cuh)
 //
 // All index arithmetic is 32 bit (a block box times 30 components stays far below 2^31).
 #pragma once
@@ -26,6 +27,7 @@
 #include <string.h>
 #include "fused_kernels.cuh"
 #include "geom_cell.cuh"
+#include "sa_tile.cuh"
 
 // tunables: threads per block / min resident blocks per SM
 #ifndef FACES_TPB
@@ -36,12 +38,6 @@
 #endif
 #ifndef FACES_MINB_SPLIT
 #define FACES_MINB_SPLIT 6
-#endif
-#ifndef SA_TPB
-#define SA_TPB 128
-#endif
-#ifndef SA_MINB
-#define SA_MINB 6
 #endif
 #ifndef NODAL_TPB
 #define NODAL_TPB 256
@@ -606,153 +602,6 @@ __global__ void __launch_bounds__(FACES_TPB, PART == 0 ? FACES_MINB : FACES_MINB
     }
 }
 
-// ---------------------------------------------------------------------------
-// SA residual pieces for one cell.
-// saAdvection, one direction: blockette.F90:1415-1560 (k), j, i analogous
-__device__ __forceinline__ double sa_adv_dir(const BlockDev& b, int N, int c, int sd, const double* __restrict__ ssum,
-                                             double voli2, double ux, double uy, double uz) {
-    const double* nt = b.w + ITU1 * N;
-    const double xa = ssum[c] * voli2, ya = ssum[N + c] * voli2, za = ssum[2 * N + c] * voli2;
-    const double uu = xa * ux + ya * uy + za * uz;
-    double dwtx;
-    if (uu > 0.0) {
-        if (c_prm.secondOrdTurb) {
-            const double dwtm1 = nt[c - sd] - nt[c - 2 * sd];
-            const double dwt = nt[c] - nt[c - sd];
-            const double dwtp1 = nt[c + sd] - nt[c];
-            dwtx = dwt;
-            if (dwt * dwtp1 > 0.0) dwtx = dwtx + 0.5 * ((fabs(dwt) < fabs(dwtp1)) ? dwt : dwtp1);
-            if (dwt * dwtm1 > 0.0) dwtx = dwtx - 0.5 * ((fabs(dwt) < fabs(dwtm1)) ? dwt : dwtm1);
-        } else {
-            dwtx = nt[c] - nt[c - sd];
-        }
-    } else {
-        if (c_prm.secondOrdTurb) {
-            const double dwtm1 = nt[c] - nt[c - sd];
-            const double dwt = nt[c + sd] - nt[c];
-            const double dwtp1 = nt[c + 2 * sd] - nt[c + sd];
-            dwtx = dwt;
-            if (dwt * dwtp1 > 0.0) dwtx = dwtx - 0.5 * ((fabs(dwt) < fabs(dwtp1)) ? dwt : dwtp1);
-            if (dwt * dwtm1 > 0.0) dwtx = dwtx + 0.5 * ((fabs(dwt) < fabs(dwtm1)) ? dwt : dwtm1);
-        } else {
-            dwtx = nt[c + sd] - nt[c];
-        }
-    }
-    return uu * dwtx;
-}
-
-// saViscous, one direction: blockette.F90:1197-1258 (k), j, i analogous.
-__device__ __forceinline__ double sa_visc_dir(const BlockDev& b, int N, int c, int sd, const double* __restrict__ s,
-                                              const double* __restrict__ ssum, double nu, double acc) {
-    const double* w = b.w;
-    const double* vol = b.vol;
-    const int cm = c - sd, cp = c + sd;
-    const double cb3Inv = c_fheat[3] /* 1 / rsaCb3 */, cb2 = c_prm.rsaCb2;
-    const double vc = vol[c];
-    const double voli = 1.0 / vc;
-    const double volmi = 2.0 / (vc + vol[cm]);
-    const double volpi = 2.0 / (vc + vol[cp]);
-    const double xm = s[cm] * volmi, ym = s[N + cm] * volmi, zm = s[2 * N + cm] * volmi;
-    const double xp = s[c] * volpi, yp = s[N + c] * volpi, zp = s[2 * N + c] * volpi;
-    const double xa = 0.5 * ssum[c] * voli, ya = 0.5 * ssum[N + c] * voli, za = 0.5 * ssum[2 * N + c] * voli;
-    const double ttm = xm * xa + ym * ya + zm * za;
-    const double ttp = xp * xa + yp * ya + zp * za;
-    const double nt0 = w[ITU1 * N + c], ntm = w[ITU1 * N + cm], ntp = w[ITU1 * N + cp];
-    const double cnud = -cb2 * nt0 * cb3Inv;
-    const double cam = ttm * cnud, cap = ttp * cnud;
-    const double nutm = 0.5 * (ntm + nt0), nutp = 0.5 * (ntp + nt0);
-    const double num = 0.5 * (b.rlv[cm] / w[cm] + nu);
-    const double nup = 0.5 * (b.rlv[cp] / w[cp] + nu);
-    const double cdm = (num + (1.0 + cb2) * nutm) * ttm * cb3Inv;
-    const double cdp = (nup + (1.0 + cb2) * nutp) * ttp * cb3Inv;
-    const double c1m = dmax_(cdm + cam, 0.0), c1p = dmax_(cdp + cap, 0.0);
-    const double c10 = c1m + c1p;
-    return acc + c1m * ntm - c10 * nt0 + c1p * ntp;
-}
-
-// saSource: blockette.F90:976-1168
-__device__ __forceinline__ double sa_source(const BlockDev& b, int N, int sJ, int sK, int c, double nu) {
-    const double* w = b.w;
-    double gv[3][3];
-#pragma unroll
-    for (int v = 0; v < 3; v++) {
-        const double* q = w + (IVX + v) * N;
-        const double qip = q[c + 1], qim = q[c - 1], qjp = q[c + sJ], qjm = q[c - sJ], qkp = q[c + sK], qkm = q[c - sK];
-#pragma unroll
-        for (int m = 0; m < 3; m++) {
-            const int o = m * N;
-            gv[v][m] = qip * b.si[o + c] - qim * b.si[o + c - 1] + qjp * b.sj[o + c] - qjm * b.sj[o + c - sJ] +
-                       qkp * b.sk[o + c] - qkm * b.sk[o + c - sK];
-        }
-    }
-    const double fact = 0.25 / b.vol[c];
-    const double sxx = 2.0 * fact * gv[0][0], syy = 2.0 * fact * gv[1][1], szz = 2.0 * fact * gv[2][2];
-    const double sxy = fact * (gv[0][1] + gv[1][0]), sxz = fact * (gv[0][2] + gv[2][0]), syz = fact * (gv[1][2] + gv[2][1]);
-    const double div2 = (2.0 * (1.0 / 3.0)) * ((sxx + syy + szz) * (sxx + syy + szz));
-    const double strainMag2 = 2.0 * (sxy * sxy + sxz * sxz + syz * syz) + sxx * sxx + syy * syy + szz * szz;
-    double sqrtProd;
-    if (c_prm.turbProd == ADFB_PROD_STRAIN) {
-        sqrtProd = sqrt(dmax_(2.0 * strainMag2 - div2, 1.e-25));
-    } else {
-        const double vortx = 2.0 * fact * (gv[2][1] - gv[1][2]);
-        const double vorty = 2.0 * fact * (gv[0][2] - gv[2][0]);
-        const double vortz = 2.0 * fact * (gv[1][0] - gv[0][1]);
-        sqrtProd = sqrt(vortx * vortx + vorty * vorty + vortz * vortz);
-    }
-    const double cv13 = c_prm.rsaCv1 * c_prm.rsaCv1 * c_prm.rsaCv1;
-    const double kar2Inv = c_fheat[4];   // 1 / rsaK**2
-    const double cw3 = c_prm.rsaCw3;
-    const double cw36 = (cw3 * cw3 * cw3) * (cw3 * cw3 * cw3);
-    const double nt = w[ITU1 * N + c];
-    const double dw_ = b.d2Wall[c];
-    const double dist2Inv = 1.0 / (dw_ * dw_);
-    const double chi = nt / nu, chi2 = chi * chi, chi3 = chi * chi2;
-    const double fv1 = chi3 / (chi3 + cv13);
-    const double fv2 = 1.0 - chi / (1.0 + chi * fv1);
-    double ft2 = 0.0;
-    if (c_prm.useft2SA) ft2 = c_prm.rsaCt3 * exp(-c_prm.rsaCt4 * chi2);
-    double sst = sqrtProd + nt * fv2 * kar2Inv * dist2Inv;
-    if (c_prm.useRotationSA) sst = sst + c_prm.rsaCrot * dmin_(0.0, sqrt(2.0 * strainMag2));
-    sst = dmax_(sst, 1.e-10);
-    double rr = nt * kar2Inv * dist2Inv / sst;
-    rr = dmin_(rr, 10.0);
-    const double rr2 = rr * rr, rr6 = rr2 * rr2 * rr2;
-    const double gg = rr + c_prm.rsaCw2 * (rr6 - rr);
-    const double gg2 = gg * gg, gg6 = gg2 * gg2 * gg2;
-    const double termFw = pow((1.0 + cw36) / (gg6 + cw36), 1.0 / 6.0);
-    const double fwSa = gg * termFw;
-    const double term1 = c_prm.rsaCb1 * (1.0 - ft2) * sqrtProd * (c_prm.approxSA ? 0.0 : 1.0);
-    const double term2 = dist2Inv * (kar2Inv * c_prm.rsaCb1 * ((1.0 - ft2) * fv2 + ft2) - c_prm.rsaCw1 * fwSa);
-    return (term1 + term2 * nt) * nt;
-}
-
-// k_sa: SA row of one owned cell: source, advection k/j/i, diffusion k/j/i, scaling
-// (blockette.F90:623-627, :1872-1897)
-// kOff / kTop: the owned planes 2 + kOff .. kTop only (slab pipeline); 0 / INT_MAX: all of them
-__global__ void __launch_bounds__(SA_TPB, SA_MINB) k_sa(Dims d, BlockDev b, MffdEpi mf, int kOff, int kTop) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x + 2;
-    const int j = blockIdx.y * blockDim.y + threadIdx.y + 2;
-    const int k = blockIdx.z * blockDim.z + threadIdx.z + 2 + kOff;
-    if (i > d.il || j > d.jl || k > d.kl || k > kTop) return;
-    const int N = (int)d.N, sJ = (int)d.sJ, sK = (int)d.sK;
-    const int c = i + sJ * j + sK * k;
-    const double rblank = dmax_((double)b.iblank[c], 0.0);
-    const double nu = b.rlv[c] / b.w[c];
-    double r = 0.0;
-    r = r + sa_source(b, N, sJ, sK, c, nu);
-    const double voli2 = 0.5 / b.vol[c];
-    const double ux = b.w[N + c], uy = b.w[2 * N + c], uz = b.w[3 * N + c];
-    r = r - sa_adv_dir(b, N, c, sK, b.ssum + 6 * N, voli2, ux, uy, uz);
-    r = r - sa_adv_dir(b, N, c, sJ, b.ssum + 3 * N, voli2, ux, uy, uz);
-    r = r - sa_adv_dir(b, N, c, 1, b.ssum, voli2, ux, uy, uz);
-    r = sa_visc_dir(b, N, c, sK, b.sk, b.ssum + 6 * N, nu, r);
-    r = sa_visc_dir(b, N, c, sJ, b.sj, b.ssum + 3 * N, nu, r);
-    r = sa_visc_dir(b, N, c, 1, b.si, b.ssum, nu, r);
-    const double dwv = -b.volRef[c] * r * rblank;
-    b.dw[ITU1 * N + c] = dwv;
-    if (mf.rec) mffd_epilogue(mf, d, i, j, k, ITU1, dwv, b.volRef[c], c_prm.turbResScale);
-}
-
 // k_div: flux divergence + sumDwandFw epilogue (blockette.F90:6839-6864) for one owned cell.
 // Order per variable: -Fi(c-1) +Fi(c) -Fj(c-sJ) +Fj(c) -Fk(c-sK) +Fk(c), like the reference's sweeps.
 template <bool MERGED>
@@ -856,29 +705,14 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     const bool gradAos = grad_aos() && flowRes && doVisc && !persistFw && !dissApprox && !viscApprox && !b.coarse && !split_faces() &&
                          !((flags & ADFB_RES_STORE_WALL) != 0) && disc == ADFB_DISS_SCALAR;
     dim3 tb(32, 4, 2);
-    // The SA row reads only the state and static geometry and writes dw(itu1); the flow rows write dw(1:5).
-    // The two chains are independent, so k_sa is forked onto a side stream (also inside graph capture) and
-    // joined at the end: both chains are latency bound, their warps interleave on the SMs.
-    static int s_conc = -1;
-    if (s_conc < 0) {
-        const char* e = getenv("ADFB_SA_CONCURRENT");
-        s_conc = e ? atoi(e) : 1;
-    }
-    const bool fork = turbRes && flowRes && s_conc && !g_kt.on;
+    // The SA row reads only the state and static geometry and writes dw(itu1); the flow rows write dw(1:5).  It runs on
+    // the same stream ahead of k_prep: the tile kernel's CTAs fill an SM's register file, so the two cannot share SMs and a
+    // side stream only added its fork and join.
     if (turbRes) {
-        dim3 tr(32, 4, 1);
-        dim3 g((d.nx + tr.x - 1) / tr.x, (d.ny + tr.y - 1) / tr.y, (d.nz + tr.z - 1) / tr.z);
-        if (fork) {
-            cudaEventRecord(env.saFork, stream);
-            cudaStreamWaitEvent(env.saStream, env.saFork, 0);
-            k_sa<<<g, tr, 0, env.saStream>>>(d, b, mf, 0, INT_MAX);
-            g_kt.launches++; g_kt.count[K_SA]++;
-            cudaEventRecord(env.saJoin, env.saStream);
-        } else {
-            KT_BEGIN(K_SA, stream);
-            k_sa<<<g, tr, 0, stream>>>(d, b, mf, 0, INT_MAX);
-            KT_END(K_SA, stream);
-        }
+        KT_BEGIN(K_SA, stream);
+        const int rc = launch_sa(d, b, env, mf, 0, INT_MAX, stream);
+        KT_END(K_SA, stream);
+        if (rc) return 1;
     }
     if (doRad || (flowRes && doDiss)) {
         dim3 g((d.NI + tb.x - 1) / tb.x, (d.NJ + tb.y - 1) / tb.y, (d.NK + tb.z - 1) / tb.z);
@@ -976,6 +810,5 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         else launch_pdl(k_div<false>, g2, tb, stream, d, b, rFil, persistFw, initWr);
         KT_END(K_DIV, stream);
     }
-    if (fork) cudaStreamWaitEvent(stream, env.saJoin, 0);
     return (int)cudaGetLastError();
 }
