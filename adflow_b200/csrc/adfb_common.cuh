@@ -101,6 +101,9 @@ __constant__ AdfbParams c_prm;
 // face and thread -- one 190-instruction pow chain per face otherwise: 21 % of the tile kernel's instructions)
 // [3] = 1/rsaCb3, [4] = 1/rsaK**2 of the SA model, [7] = 1/(gamma-1), [8] = 1e-6 gamma pInfCorr / rhoInf (host quotients: correctly
 // rounded on both sides); [5] = rhoInf**gamma / pInfCorr, [6] = sqrt(gamma pInfCorr / rhoInf) of the far-field BC (device)
+// [9], [10]: the second-difference coefficients of the scalar dissipation, vis2 itself without dissipation-based continuation;
+// with it [9] is that of inviscidDissFluxScalar (zero guard on totalR, totalR0) and [10] that of ...ScalarApprox (no guard).
+// Formed on the host in the reference's expression order whenever the parameters or the total residuals change.
 __constant__ double c_fheat[16];
 // Programmatic dependent launch: every PDL-launched kernel first waits for its predecessor (grid dependency sync: the
 // predecessor has completed and its writes are visible), then -- with ADFB_PDL_TRIGGER=1 -- signals at once that ITS

@@ -47,6 +47,7 @@ struct Block {
     int32_t* dOrphans = nullptr;
     double muInf = 0.0, eddyVisInfRatio = 0.0;
     std::vector<void*> mgAllocs;
+    double* saved = nullptr;   // w, p, rlv, rev kept by adfb_free_stream_residual (in allocs)
 };
 
 struct Context {
@@ -120,6 +121,7 @@ struct Context {
     size_t kryVN = 0;
     int mgInitWr = 1;   // coarse-level smoother residual starts from wr (0 inside transferToCoarseGrid: from zero)
     int groundLevel = 1;   // iteration%groundLevel: the finest level of the current multigrid cycle (> 1 during the full-multigrid start-up)
+    double totalR = 0.0, totalR0 = 0.0;   // iteration%totalR, totalR0 (adfb_set_total_residuals)
 };
 
 Context g;
@@ -287,6 +289,21 @@ void drop_comm_tables() {
     for (auto* m : {&g.pats, &g.ovPats})
         for (auto& kv : *m) kv.second.tabs.clear();
 }
+// The two second-difference coefficients of the scalar dissipation (c_fheat[9], [10]) for the current parameters and total
+// residuals, in double on the host with the reference's expression order, so that rFil * fis2 has the reference's bits.
+void diss_coefs(double out[2]) {
+    const AdfbParams& P = g.prm;
+    out[0] = out[1] = P.vis2;
+    if (!P.useDissContinuation) return;
+    // inviscidDissFluxScalar (blockette.F90:3114-3123, fluxes.F90:1176-1185): log10 of a zero ratio is avoided
+    if (g.totalR == 0.0 || g.totalR0 == 0.0)
+        out[0] = P.vis2 + P.dissContMagnitude / (1 + exp(-P.dissContSharpness * P.dissContMidpoint));
+    else
+        out[0] = P.vis2 + P.dissContMagnitude / (1 + exp(-P.dissContSharpness * (log10(g.totalR / g.totalR0) + P.dissContMidpoint)));
+    // inviscidDissFluxScalarApprox (blockette.F90:4434-4439) has no such guard: totalR = 0 gives vis2, both zero NaN
+    out[1] = P.vis2 + P.dissContMagnitude / (1 + exp(-P.dissContSharpness * (log10(g.totalR / g.totalR0) + P.dissContMidpoint)));
+}
+
 void drop_graphs() {
     drop_comm_tables();
     for (auto& kv : g.graphs) cudaGraphExecDestroy(kv.second);
@@ -419,6 +436,7 @@ int adfb_finalize(void) {
     // so do the parameters and the multigrid position: a later context starts on ground level 1 and must set its parameters
     g.havePrm = false;
     g.groundLevel = 1; g.mgInitWr = 1;
+    g.totalR = 0.0; g.totalR0 = 0.0;
     for (auto* M : {&g.pats, &g.ovPats}) {
         for (auto& kv : *M) for (void* q : kv.second.allocs) cudaFree(q);
         M->clear();
@@ -481,6 +499,7 @@ int adfb_set_params(const AdfbParams* prm) {
         fheat[0] = 1.0 / (g.prm.prandtl * gm1); fheat[1] = 1.0 / (g.prm.prandtlTurb * gm1);
         fheat[3] = 1.0 / g.prm.rsaCb3; fheat[4] = 1.0 / (g.prm.rsaK * g.prm.rsaK);
         fheat[7] = 1.0 / gm1; fheat[8] = 0.000001 * g.prm.gammaInf * g.prm.pInfCorr / g.prm.rhoInf;
+        diss_coefs(fheat + 9);
         CK(cudaMemcpyToSymbolAsync(c_fheat, fheat, sizeof fheat, 0, cudaMemcpyHostToDevice, g.stream));
         k_param_consts<<<1, 1, 0, g.stream>>>(g.dConst);   // reads the c_prm uploaded above (stream order)
         CK(cudaMemcpyToSymbolAsync(c_fheat, g.dConst, sizeof(double), 2 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
@@ -2428,6 +2447,42 @@ int adfb_norms(double out[2]) {
         out[0] = g.hRed[0]; out[1] = g.hRed[1];
     }
     return 0;
+}
+
+int adfb_set_total_residuals(double totalR, double totalR0) {
+    NEED_INIT();
+    g.totalR = totalR; g.totalR0 = totalR0;
+    if (!g.havePrm) return 0;   // adfb_set_params forms the coefficients from these values
+    // the kernels read the coefficients from constant memory when they run: the recorded graphs stay valid, and the copy
+    // is ordered on the library stream before any later work
+    double coef[2];
+    diss_coefs(coef);
+    CK(cudaMemcpyToSymbolAsync(c_fheat, coef, sizeof coef, 9 * sizeof(double), cudaMemcpyHostToDevice, g.stream));
+    return 0;
+}
+
+// getFreeStreamResidual (NKSolvers.F90:280-333) on the level-1 blocks: getInfo / setInfo keep w, p, rlv, rev in a device
+// copy of the block's state slab (allocated on first use, freed with the block)
+int adfb_free_stream_residual(double out[2]) {
+    ADFB_RANGE("adfb_free_stream_residual");
+    NEED_INIT();
+    if (!out) return fail("adfb_free_stream_residual: null");
+    if (!g.havePrm) return fail("adfb_free_stream_residual: adfb_set_params has not been called");
+    const unsigned flags = ADFB_RES_FLOW | ADFB_RES_TURB | ADFB_RES_UPDATE_INTERMED;
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != 1) continue;
+        const size_t n = (size_t)b.d.N * (b.nw + 3);   // w(nw), p, rlv, rev: one contiguous slab
+        if (!b.saved && dalloc(b, &b.saved, n)) return 1;
+        CK(cudaMemcpyAsync(b.saved, b.dev.w, n * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
+        if (launch_vec(b.d, b.dev, b.nw, nullptr, 3, g.stream)) return fail("free-stream state kernel launch failed");
+    }
+    if (adfb_residual(1, flags) || adfb_norms(out)) return 1;
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != 1) continue;
+        CK(cudaMemcpyAsync(b.dev.w, b.saved, (size_t)b.d.N * (b.nw + 3) * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
+    }
+    // the reference evaluates the residual of the restored state once more (NKSolvers.F90:327-331)
+    return adfb_residual(1, flags);
 }
 
 // getForces / wallIntegrationFace: Fp(3), Fv(3), Mp(3), Mv(3) over the wall subfaces of all local blocks of

@@ -158,7 +158,12 @@ FHD void ff_cons(const FCell& s, double Q[5]) {
 // scalar JST (inviscidDissFluxScalar, blockette.F90:3133-3338); Qmm / Qqq: conservative variables of c-sd / cp+sd
 FHD void ff_jst(const AdfbParams& P, const double Qmm[5], const FCell& m, const FCell& q, const double Qqq[5], int por,
                 double radSum, double dssMax, double rFil, double fd[5]) {
-    const double fis2 = rFil * P.vis2, fis4 = rFil * P.vis4;
+#if defined(__CUDA_ARCH__)
+    const double vis2 = c_fheat[9];   // vis2, with dissipation-based continuation when it is on (adfb_set_total_residuals)
+#else
+    const double vis2 = P.vis2;       // the CPU emulation runs without continuation
+#endif
+    const double fis2 = rFil * vis2, fis4 = rFil * P.vis4;
     const double ppor = (por == ADFB_NORMALFLUX) ? 0.5 : 0.0;
     const double rrad = ppor * radSum;
     const double dis2 = fis2 * rrad * dmin_(0.25, dssMax);

@@ -283,7 +283,7 @@ __device__ __forceinline__ void face_flux(const BlockDev& b, int N, int c, int s
     }
     if (DISC == ADFB_DISS_SCALAR && !(APPROX & 5) && doDiss) {  // scalar JST
         const CellState mm = load_cell(b, N, c - sd), qq = load_cell(b, N, cp + sd);
-        const double fis2 = rFil * c_prm.vis2, fis4 = rFil * c_prm.vis4;
+        const double fis2 = rFil * c_fheat[9] /* vis2, with continuation */, fis4 = rFil * c_prm.vis4;
         const double ppor = (por == ADFB_NORMALFLUX) ? 0.5 : 0.0;
         const double rrad = ppor * (rad[c] + rad[cp]);
         const double dis2 = fis2 * rrad * dmin_(0.25, dmax_(dss[c], dss[cp]));
@@ -302,7 +302,8 @@ __device__ __forceinline__ void face_flux(const BlockDev& b, int N, int c, int s
     if (DISC == ADFB_DISS_SCALAR && (APPROX & 1) && !(APPROX & 4) && doDiss) {  // inviscidDissFluxScalarApprox, blockette.F90:4367-4617
         const double ppor = (por == ADFB_NORMALFLUX) ? 0.5 : 0.0;
         const double rrad = ppor * (rad[c] + rad[cp]);
-        const double dis2 = c_prm.vis2 * rrad * dmin_(0.25, dmax_(dss[c], dss[cp])) + c_prm.sigma * c_prm.vis4 * rrad;
+        const double dis2 = c_fheat[10] /* vis2, with continuation */ * rrad * dmin_(0.25, dmax_(dss[c], dss[cp])) +
+                            c_prm.sigma * c_prm.vis4 * rrad;
         fd[0] = dis2 * (q.r - m.r);
         fd[1] = dis2 * (q.u * q.r - m.u * m.r);
         fd[2] = dis2 * (q.v * q.r - m.v * m.r);

@@ -144,10 +144,15 @@ __global__ void __launch_bounds__(256) k_norms_final(double* part, int nPart) {
 }
 
 // AoS <-> SoA vector kernels (getStates/setStates/getRes gather loops,
-// src/NKSolver/NKSolvers.F90:1378-1485). mode 0: vec <- w ; 1: w <- vec ; 2: vec <- dw/volRef
+// src/NKSolver/NKSolvers.F90:1378-1485). mode 0: vec <- w ; 1: w <- vec ; 2: vec <- dw/volRef ;
+// 3: w(0:ib, 0:jb, 0:kb, 1:nw) <- wInf, halos included (the uniform flow of getFreeStreamResidual, :298-312; vec unused)
 __global__ void __launch_bounds__(256) k_vec(Dims d, BlockDev b, int nw, double* vec, int mode) {
     const long long nOwned = (long long)d.nx * d.ny * d.nz;
     const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (mode == 3) {
+        if (q < d.N * nw) b.w[q] = c_prm.wInf[q / d.N];
+        return;
+    }
     if (q >= nOwned * nw) return;
     const int l = (int)(q % nw);
     const long long cell = q / nw;
@@ -256,7 +261,7 @@ __global__ void __launch_bounds__(256) k_sum_final(double* part, int nPart) {
 }  // namespace
 
 static int launch_vec(const Dims& d, const BlockDev& b, int nw, double* vec, int mode, cudaStream_t stream) {
-    const long long n = (long long)d.nx * d.ny * d.nz * nw;
+    const long long n = (mode == 3 ? d.N : (long long)d.nx * d.ny * d.nz) * nw;   // mode 3 covers the whole box
     KT_BEGIN(K_VEC, stream);
     k_vec<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d, b, nw, vec, mode);
     KT_END(K_VEC, stream);

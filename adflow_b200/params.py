@@ -42,6 +42,8 @@ class AdfbParams(C.Structure):
         ("nSubiterTurb", C.c_int32), ("wallBCConstantPressure", C.c_int32), ("reserved", C.c_int32),
         ("hScalingInlet", C.c_int32), ("outflowLinearExtrapol", C.c_int32),
         ("mgBoundCorr", C.c_int32), ("spaceDiscrCoarse", C.c_int32),
+        ("useDissContinuation", C.c_int32), ("pad_", C.c_int32),
+        ("dissContMagnitude", C.c_double), ("dissContMidpoint", C.c_double), ("dissContSharpness", C.c_double),
     ]
 
 
@@ -105,6 +107,10 @@ DEFAULT_OPTIONS = {
     "useApproxSA": False,
     "limiter": "van Albada",
     "kappaCoef": 1.0 / 3.0,
+    "useDissContinuation": False,
+    "dissContMagnitude": 1.0,
+    "dissContMidpoint": 3.0,
+    "dissContSharpness": 3.0,
 }
 
 
@@ -252,5 +258,8 @@ def make_params(options=None, mach=0.8, alpha_deg=1.8, P=20000.0, T=220.0, R=287
     prm.resAveraging = {"never": 0, "always": 1, "alternate": 2}[opt["resAveraging"]]
     prm.nSubiterTurb = opt["nSubiterTurb"]
     prm.wallBCConstantPressure = int(opt["viscWallTreatment"] == "constant pressure extrapolation")
+    prm.useDissContinuation = int(opt["useDissContinuation"])
+    prm.dissContMagnitude, prm.dissContMidpoint = opt["dissContMagnitude"], opt["dissContMidpoint"]
+    prm.dissContSharpness = opt["dissContSharpness"]
     prm._muInf = muInf  # convenience for the synthetic-state generator (not part of the POD)
     return prm

@@ -362,6 +362,17 @@ class ADFLOW_B200:
         check(self.L.adfb_norms(out), "adfb_norms")
         return np.array([out[0], out[1]])
 
+    def getFreeStreamResidual(self):
+        """totalR0: the L2 norm of the residual of the uniform free stream on the fine grid (pyADflow.py:5422-5425,
+        getFreeStreamResidual NKSolvers.F90:280-333); the state on the device is left as it was."""
+        out = (C.c_double * 2)()
+        check(self.L.adfb_free_stream_residual(out), "adfb_free_stream_residual")
+        return float(np.sqrt(out[1]))
+
+    def setTotalResiduals(self, totalR, totalR0):
+        """iteration%totalR and totalR0, read by the dissipation-based continuation (useDissContinuation)."""
+        check(self.L.adfb_set_total_residuals(float(totalR), float(totalR0)), "adfb_set_total_residuals")
+
     def getForces(self, ref_point=(0.0, 0.0, 0.0), p_ref=1.0, level=1):
         """Fp, Fv, Mp, Mv (rows) summed over the wall subfaces of all ranks -- wallIntegrationFace,
         src/solver/surfaceIntegrations.F90:406-881.  Call residual(flags | RES_STORE_WALL) first (as the

@@ -134,6 +134,14 @@ typedef struct AdfbParams {
     int32_t outflowLinearExtrapol; /* outflowTreatment == linExtrapol (default constantExtrapol), supersonic outflow */
     int32_t mgBoundCorr;           /* 0 = bcDirichlet0 (default), 1 = bcNeumann0: boundary halos of the interpolated corrections */
     int32_t spaceDiscrCoarse;      /* coarse-level discretisation: ADFB_DISS_SCALAR or ADFB_DISS_MATRIX on levels > 1 */
+    /* dissipation-based continuation (inputIteration useDissContinuation, dissContMagnitude, dissContMidpoint,
+       dissContSharpness): the second-difference coefficient of the scalar dissipation becomes
+       vis2 + dissContMagnitude / (1 + exp(-dissContSharpness * (log10(totalR / totalR0) + dissContMidpoint)))
+       with totalR, totalR0 of adfb_set_total_residuals (blockette.F90:3114-3123, 4434-4439, fluxes.F90:1176-1185).
+       No effect with matrix dissipation, upwinding or on the coarse levels of multigrid, as in the reference. */
+    int32_t useDissContinuation;
+    int32_t pad_;
+    double dissContMagnitude, dissContMidpoint, dissContSharpness;
 } AdfbParams;
 
 /* One boundary subface of a block, mirroring BCDataType (src/modules/block.F90:52-156)
@@ -213,6 +221,16 @@ int adfb_residual(int level, unsigned flags);
 /* Sum of (dw(irho)/vol)^2 and of all (dw/vol)^2 over owned cells of all local
    blocks, all-reduced (getCurrentResidual, NKSolvers.F90:335-370). out[0]=rho, out[1]=total */
 int adfb_norms(double out[2]);
+/* iteration%totalR and totalR0 (convergenceInfo, solvers.F90:1672; getFreeStreamResidual): the L2 norm of the current
+   residual and of the free-stream residual, the same all-reduced values on every rank.  Only the dissipation-based
+   continuation reads them; the host calls this after its convergence monitor and after adfb_free_stream_residual.
+   A context starts with 0 and 0.  Cheap between cycles: recorded CUDA graphs stay valid. */
+int adfb_set_total_residuals(double totalR, double totalR0);
+/* getFreeStreamResidual (NKSolvers.F90:280-333): on every level-1 block, w(:,:,:,1:nw) = wInf including both halo
+   layers, adfb_residual(1, FLOW | TURB | UPDATE_INTERMED), the sums of adfb_norms (out[0] rho, out[1] total,
+   all-reduced), then w, p, rlv, rev restored and the same residual evaluated again, as the reference does.  The host
+   takes totalR0 = sqrt(out[1]). */
+int adfb_free_stream_residual(double out[2]);
 /* blocks until the library stream is idle (the reference is synchronous: needed only before timing or host reads
    that bypass the download calls) */
 int adfb_synchronize(void);
