@@ -18,7 +18,7 @@ ABI_SYMBOLS = [
     "adfb_block_create", "adfb_block_destroy", "adfb_block_set_geometry", "adfb_block_set_bc",
     "adfb_set_params", "adfb_upload_state", "adfb_download_state", "adfb_upload_visc",
     "adfb_download_residual", "adfb_download_intermed", "adfb_residual", "adfb_norms", "adfb_synchronize", "adfb_forces",
-    "adfb_set_total_residuals", "adfb_free_stream_residual",
+    "adfb_set_total_residuals", "adfb_free_stream_residual", "adfb_inf_change_correction", "adfb_set_uniform_flow",
     "adfb_get_states", "adfb_set_states", "adfb_get_res", "adfb_state_size",
     "adfb_comm_set_pattern", "adfb_comm_set_overset", "adfb_block_set_orphans", "adfb_halo_exchange",
     "adfb_reference_shock_sensor", "adfb_form_function", "adfb_mffd_set_base", "adfb_mffd_apply", "adfb_mffd_apply_device", "adfb_mffd_last_h",
@@ -80,6 +80,8 @@ def load():
     L.adfb_norms.argtypes = [C.POINTER(C.c_double)]
     L.adfb_set_total_residuals.argtypes = [C.c_double, C.c_double]
     L.adfb_free_stream_residual.argtypes = [C.POINTER(C.c_double)]
+    L.adfb_inf_change_correction.argtypes = [C.POINTER(C.c_double), C.c_double, ci, C.POINTER(ci)]
+    L.adfb_set_uniform_flow.argtypes = [ci, C.c_double, C.c_double]
     L.adfb_forces.argtypes = [ci, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_double)]
     for fn in (L.adfb_get_states, L.adfb_set_states, L.adfb_get_res):
         fn.argtypes = [vp, C.c_longlong]

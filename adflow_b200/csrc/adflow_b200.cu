@@ -2485,6 +2485,95 @@ int adfb_free_stream_residual(double out[2]) {
     return adfb_residual(1, flags);
 }
 
+// myNorm2 (utils.F90:1696-1702): a dimension(3) dummy, so only the first three entries count
+static double my_norm2(const double x[3]) { return sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]); }
+
+// getRotMatrix (utils.F90:6591-6665): Rodrigues' formula for the rotation of the direction of v1 to that of v2, in the
+// reference's expression order (matmul sums from zero in index order).  rot[3 (i-1) + (j-1)] = rotMat(i, j).
+static void rot_matrix(const double v1[3], const double v2[3], double rot[9]) {
+    double dotProd = 0.0;
+    for (int i = 0; i < 3; i++) dotProd = dotProd + v1[i] * v2[i];
+    const double mag1 = my_norm2(v1), mag2 = my_norm2(v2);
+    const double cosine = dotProd / (mag1 * mag2);
+    const double theta = acos(cosine);
+    double v3[3] = {v1[1] * v2[2] - v1[2] * v2[1], v1[2] * v2[0] - v1[0] * v2[2], v1[0] * v2[1] - v1[1] * v2[0]};
+    const double len = sqrt(v3[0] * v3[0] + v3[1] * v3[1] + v3[2] * v3[2]);
+    for (int i = 0; i < 3; i++) v3[i] = v3[i] / len;
+    double W[3][3] = {{0.0, -v3[2], v3[1]}, {v3[2], 0.0, -v3[0]}, {-v3[1], v3[0], 0.0}};
+    const double s = sin(theta), c = 1.0 - cos(theta);
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            double w2 = 0.0;
+            for (int k = 0; k < 3; k++) w2 = w2 + W[i][k] * W[k][j];
+            rot[3 * i + j] = ((i == j ? 1.0 : 0.0) + s * W[i][j]) + c * w2;
+        }
+}
+
+// infChangeCorrection (src/initFlow/initializeFlow.F90:191-316) on the level-1 blocks, the new free stream being the wInf of
+// the last adfb_set_params.  See include/adflow_b200.h for the refusals; each leaves the state as it was.
+int adfb_inf_change_correction(const double oldWinf[5], double tol, int type, int* applied) {
+    ADFB_RANGE("adfb_inf_change_correction");
+    NEED_INIT();
+    if (!oldWinf || !applied) return fail("adfb_inf_change_correction: null");
+    *applied = 0;
+    if (!g.havePrm) return fail("adfb_inf_change_correction: adfb_set_params has not been called");
+    if (type != 0 && type != 1) return fail("adfb_inf_change_correction: unknown correction type %d (0 offset, 1 rotate)", type);
+    // the reference corrects level 1 and exchanges on currentLevel: the two agree only on ground level 1
+    if (g.groundLevel != 1) return fail("adfb_inf_change_correction: ground level is %d, not 1", g.groundLevel);
+    VecCoef cf = {};
+    for (int l = 0; l < 5; l++) cf.dWinf[l] = g.prm.wInf[l] - oldWinf[l];
+    if (my_norm2(cf.dWinf) < tol) return 0;   // rho, u, v only (myNorm2): nothing is launched
+    if (type == 1) {
+        rot_matrix(oldWinf + 1, g.prm.wInf + 1, cf.rot);
+        cf.mag1 = my_norm2(oldWinf + 1);
+        cf.mag2 = my_norm2(g.prm.wInf + 1);
+        bool finite = std::isfinite(cf.mag1) && std::isfinite(cf.mag2) && std::isfinite(cf.mag2 / cf.mag1);
+        for (double r : cf.rot) finite = finite && std::isfinite(r);
+        // a change of speed alone gives vec1 x vec2 = 0: the reference normalises 0 / 0 and writes NaN into every velocity
+        if (!finite)
+            return fail("adfb_inf_change_correction: \"rotate\" has no finite rotation for this change of the free stream "
+                        "(the velocity direction is unchanged or a velocity is zero); use \"offset\"");
+    }
+    const bool rans = g.prm.equations == ADFB_RANS;
+    const int nwAll = rans ? 6 : 5;   // flowVarRefState nw: the same exchanged range on every rank, whatever its blocks
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != 1) continue;
+        if (launch_vec(b.d, b.dev, b.nw, nullptr, type == 0 ? 4 : 5, g.stream, cf)) return fail("correction kernel launch failed");
+        // applyAllBC_block(.true.) from the corrected w and the pressure as it was: the reference does not recompute p first
+        if (launch_bc_levels(b.d, b.dev, b.subfaces, 1, 0, 1, g.stream)) return fail("flow BC launch failed");
+    }
+    // whalo2(currentLevel, 1, nw, .true., .true., .true.): exchange, orphan averaging, owned-cell total energy
+    if (halo_exchange_impl(1, 1, nwAll, 1, 1, true)) return 1;
+    if (overset_present(1)) {
+        // BC halos behind interpolated cells follow the interpolated values: turbulence (RANS) and flow BCs again
+        for (Block& b : g.blocks) {
+            if (!b.alive || b.level != 1) continue;
+            if (launch_bc_levels(b.d, b.dev, b.subfaces, 1, rans ? 1 : 0, 1, g.stream)) return fail("BC launch failed");
+        }
+    }
+    CK(cudaGetLastError());
+    *applied = 1;
+    return 0;
+}
+
+// setUniformFlow (initializeFlow.F90:2143-2212) on the blocks of `level` (mgStartLevel), halos included
+int adfb_set_uniform_flow(int level, double muInf, double eddyVisInfRatio) {
+    ADFB_RANGE("adfb_set_uniform_flow");
+    NEED_INIT();
+    if (!g.havePrm) return fail("adfb_set_uniform_flow: adfb_set_params has not been called");
+    bool have = false;
+    for (Block& b : g.blocks) if (b.alive && b.level == level) have = true;
+    if (!have) return fail("adfb_set_uniform_flow: no block of level %d", level);
+    VecCoef cf = {};
+    cf.muInf = muInf;
+    cf.revInf = eddyVisInfRatio * muInf;
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != level) continue;
+        if (launch_vec(b.d, b.dev, b.nw, nullptr, 6, g.stream, cf)) return fail("uniform-flow kernel launch failed");
+    }
+    return 0;
+}
+
 // getForces / wallIntegrationFace: Fp(3), Fv(3), Mp(3), Mv(3) over the wall subfaces of all local blocks of
 // `level`, all-reduced.  The viscous part uses the wall stresses stored by the last adfb_residual call that had
 // ADFB_RES_STORE_WALL set.

@@ -143,14 +143,58 @@ __global__ void __launch_bounds__(256) k_norms_final(double* part, int nPart) {
     if (threadIdx.x == 0) { part[2 * nPart] = s0[0]; part[2 * nPart + 1] = s1[0]; }
 }
 
+// The per-call coefficients of the whole-state modes of k_vec, formed on the host: the free-stream change and the rotation
+// of infChangeCorrection (modes 4, 5), the free-stream viscosities of setUniformFlow (mode 6)
+struct VecCoef {
+    double dWinf[5];     // wInf(1:5) - oldWinf
+    double rot[9];       // rotMat(i, j) at [3 (i-1) + (j-1)] (getRotMatrix)
+    double mag1, mag2;   // |old velocity|, |new velocity|
+    double muInf, revInf;
+};
+
 // AoS <-> SoA vector kernels (getStates/setStates/getRes gather loops,
 // src/NKSolver/NKSolvers.F90:1378-1485). mode 0: vec <- w ; 1: w <- vec ; 2: vec <- dw/volRef ;
-// 3: w(0:ib, 0:jb, 0:kb, 1:nw) <- wInf, halos included (the uniform flow of getFreeStreamResidual, :298-312; vec unused)
-__global__ void __launch_bounds__(256) k_vec(Dims d, BlockDev b, int nw, double* vec, int mode) {
+// 3: w(0:ib, 0:jb, 0:kb, 1:nw) <- wInf, halos included (the uniform flow of getFreeStreamResidual, :298-312; vec unused).
+// Whole-state modes (vec unused, coefficients in cf):
+// 4: w(2:il, 2:jl, 2:kl, 1:5) += dWinf, one thread per owned cell ("offset" of infChangeCorrection,
+//    src/initFlow/initializeFlow.F90:230-247)
+// 5: owned velocity <- (rot v) * mag2 / mag1, rho and rhoE += their dWinf ("rotate", :249-284); explicit roundings, so that
+//    no FMA contraction changes the reference's bits
+// 6: setUniformFlow (:2143-2212) over the whole box, one thread per cell: w = wInf, dw = 0, fw = 0, p = pInfCorr,
+//    rlv = muInf unless Euler, rev = eddyVisInfRatio * muInf for RANS
+__global__ void __launch_bounds__(256) k_vec(Dims d, BlockDev b, int nw, double* vec, int mode, VecCoef cf) {
     const long long nOwned = (long long)d.nx * d.ny * d.nz;
     const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (mode == 3) {
         if (q < d.N * nw) b.w[q] = c_prm.wInf[q / d.N];
+        return;
+    }
+    if (mode == 6) {
+        if (q >= d.N) return;
+        for (int l = 0; l < nw; l++) { b.w[l * d.N + q] = c_prm.wInf[l]; b.dw[l * d.N + q] = 0.0; }
+        for (int l = 0; l < 5; l++) b.fw[l * d.N + q] = 0.0;
+        b.p[q] = c_prm.pInfCorr;
+        if (c_prm.equations != ADFB_EULER) b.rlv[q] = cf.muInf;
+        if (c_prm.equations == ADFB_RANS) b.rev[q] = cf.revInf;
+        return;
+    }
+    if (mode >= 4) {
+        if (q >= nOwned) return;
+        const long long c = ADFB_IDX((int)(q % d.nx) + 2, (int)((q / d.nx) % d.ny) + 2, (int)(q / ((long long)d.nx * d.ny)) + 2);
+        const long long N = d.N;
+        if (mode == 4) {
+            for (int l = 0; l < 5; l++) b.w[l * N + c] = __dadd_rn(b.w[l * N + c], cf.dWinf[l]);
+            return;
+        }
+        const double v[3] = {b.w[N + c], b.w[2 * N + c], b.w[3 * N + c]};
+        for (int m = 0; m < 3; m++) {
+            // matmul(rotMat, vCell): ((r1 v1 + r2 v2) + r3 v3), then * mag2, then / mag1
+            const double r = __dadd_rn(__dadd_rn(__dmul_rn(cf.rot[3 * m], v[0]), __dmul_rn(cf.rot[3 * m + 1], v[1])),
+                                       __dmul_rn(cf.rot[3 * m + 2], v[2]));
+            b.w[(m + 1) * N + c] = __ddiv_rn(__dmul_rn(r, cf.mag2), cf.mag1);
+        }
+        b.w[c] = __dadd_rn(b.w[c], cf.dWinf[0]);
+        b.w[4 * N + c] = __dadd_rn(b.w[4 * N + c], cf.dWinf[4]);
         return;
     }
     if (q >= nOwned * nw) return;
@@ -260,10 +304,13 @@ __global__ void __launch_bounds__(256) k_sum_final(double* part, int nPart) {
 
 }  // namespace
 
-static int launch_vec(const Dims& d, const BlockDev& b, int nw, double* vec, int mode, cudaStream_t stream) {
-    const long long n = (mode == 3 ? d.N : (long long)d.nx * d.ny * d.nz) * nw;   // mode 3 covers the whole box
+static int launch_vec(const Dims& d, const BlockDev& b, int nw, double* vec, int mode, cudaStream_t stream,
+                      const VecCoef& cf = VecCoef()) {
+    const long long nOwned = (long long)d.nx * d.ny * d.nz;
+    // mode 3 covers the whole box per variable, 4 and 5 the owned cells, 6 the box cells
+    const long long n = mode == 3 ? d.N * nw : mode == 6 ? d.N : mode >= 4 ? nOwned : nOwned * nw;
     KT_BEGIN(K_VEC, stream);
-    k_vec<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d, b, nw, vec, mode);
+    k_vec<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d, b, nw, vec, mode, cf);
     KT_END(K_VEC, stream);
     return (int)cudaGetLastError();
 }

@@ -369,6 +369,32 @@ class ADFLOW_B200:
         check(self.L.adfb_free_stream_residual(out), "adfb_free_stream_residual")
         return float(np.sqrt(out[1]))
 
+    INF_CHANGE_TYPES = {"offset": 0, "rotate": 1}
+
+    def infChangeCorrection(self, old_winf, tol=1e-12, kind="offset"):
+        """infChangeCorrection (initializeFlow.F90:191-316, pyADflow.py:3416-3421): correct the state of the level-1 blocks
+        from the free stream old_winf (its first five entries) to the wInf of the current parameters (setParams first).
+        kind is pyADflow's infChangeCorrectionType, "offset" or "rotate".  Returns whether the state was changed: a change
+        whose rho, u, v part is below tol is skipped, as in the reference."""
+        if kind not in self.INF_CHANGE_TYPES:
+            raise ValueError("infChangeCorrection: kind must be 'offset' or 'rotate', got %r" % (kind,))
+        old = (C.c_double * 5)(*[float(v) for v in list(old_winf)[:5]])
+        applied = C.c_int(0)
+        check(self.L.adfb_inf_change_correction(old, float(tol), self.INF_CHANGE_TYPES[kind], C.byref(applied)),
+              "adfb_inf_change_correction")
+        return bool(applied.value)
+
+    def setUniformFlow(self, level, mu_inf, eddy_vis_inf_ratio):
+        """setUniformFlow (initializeFlow.F90:2143-2212) on the blocks of `level`: w = wInf, dw = fw = 0, p = pInfCorr,
+        rlv = mu_inf (viscous), rev = eddy_vis_inf_ratio * mu_inf (RANS), halos included."""
+        check(self.L.adfb_set_uniform_flow(level, float(mu_inf), float(eddy_vis_inf_ratio)), "adfb_set_uniform_flow")
+
+    def resetFlow(self, mg_start_level, mu_inf, eddy_vis_inf_ratio):
+        """_resetFlow (pyADflow.py:3097-3111): the ground level becomes mgStartLevel and its blocks get the uniform flow;
+        fullMultigridStartUp(mg_start_level, ...) then starts from there."""
+        self.setGroundLevel(mg_start_level)
+        self.setUniformFlow(mg_start_level, mu_inf, eddy_vis_inf_ratio)
+
     def setTotalResiduals(self, totalR, totalR0):
         """iteration%totalR and totalR0, read by the dissipation-based continuation (useDissContinuation)."""
         check(self.L.adfb_set_total_residuals(float(totalR), float(totalR0)), "adfb_set_total_residuals")

@@ -231,6 +231,25 @@ int adfb_set_total_residuals(double totalR, double totalR0);
    all-reduced), then w, p, rlv, rev restored and the same residual evaluated again, as the reference does.  The host
    takes totalR0 = sqrt(out[1]). */
 int adfb_free_stream_residual(double out[2]);
+/* infChangeCorrection (src/initFlow/initializeFlow.F90:191-316): correct the state of every level-1 block from the free
+   stream oldWinf(1:5) to the wInf of the last adfb_set_params, as pyADflow's setAeroProblem does when a solved
+   AeroProblem changes its Mach number, angles, pressure or temperature (pyADflow.py:3416-3421).
+   deltaWinf = wInf(1:5) - oldWinf.  If sqrt(deltaWinf(1)^2 + deltaWinf(2)^2 + deltaWinf(3)^2) < tol -- myNorm2 takes a
+   dimension(3) dummy, so only rho, u, v are measured -- nothing is launched and *applied = 0.  Otherwise, on the owned
+   cells: type 0 ("offset") adds deltaWinf to w(1:5); type 1 ("rotate") rotates the velocity by getRotMatrix(old, new
+   velocity) (utils.F90:6591-6665), scales it by |new| / |old| and adds the offsets of rho and rho E.  The turbulence
+   variable is not touched.  Then the flow BCs with second halos on every block, from the corrected w and the pressure
+   as it was (the reference does not recompute p first), whalo2(1, 1, nw, T, T, T) with orphan averaging and the
+   owned-cell total energy, and with an overset pattern the turbulence (RANS) and flow BCs again; *applied = 1.
+   Refused (non-zero return, adfb_last_error, state untouched): a null pointer, no adfb_set_params, an unknown type,
+   ground level other than 1, and "rotate" without a finite rotation (a change of speed alone makes vec1 x vec2 = 0,
+   where the reference writes NaN into every velocity). */
+int adfb_inf_change_correction(const double oldWinf[5], double tol, int type, int* applied);
+/* setUniformFlow (initializeFlow.F90:2143-2212) on every block of `level` (mgStartLevel), halos included: w(1:nw) = wInf,
+   dw = 0, fw = 0, p = pInfCorr, rlv = muInf unless Euler, rev = eddyVisInfRatio * muInf for RANS.  muInf and
+   eddyVisInfRatio are flowVarRefState / inputPhysics values, passed as in adfb_block_set_orphans.  The time-spectral
+   internal-flow branch (:2213-2286) is not built.  Fails if no block of `level` exists. */
+int adfb_set_uniform_flow(int level, double muInf, double eddyVisInfRatio);
 /* blocks until the library stream is idle (the reference is synchronous: needed only before timing or host reads
    that bypass the download calls) */
 int adfb_synchronize(void);
