@@ -383,6 +383,13 @@ int adfb_init(int device, const void* ncclUniqueId, int rank, int nranks) {
     {
         int v = 0;
         CK(cudaDeviceGetAttribute(&g.env.nSM, cudaDevAttrMultiProcessorCount, device));
+        // ADFB_SM_COUNT=n (tests): the launch choosers (ftile_choose, sa_tile_choose, lines_per_cta) plan for n
+        // multiprocessors, so that small blocks get the long k chunks and full line tables of large ones.  Every pick is
+        // a legal launch: no kernel assumes co-resident CTAs.
+        if (const char* e = getenv("ADFB_SM_COUNT")) {
+            const int n = atoi(e);
+            if (n >= 1 && n < g.env.nSM) g.env.nSM = n;
+        }
         CK(cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         g.env.smemOptin = (size_t)v;
         // the kernels that take more dynamic shared memory than the default 48 KiB

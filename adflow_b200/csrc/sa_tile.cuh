@@ -21,6 +21,8 @@
 #pragma once
 #include "adfb_common.cuh"
 #include <math.h>
+#include <stdio.h>
+#include <stdlib.h>
 
 #if defined(__CUDACC__)
 #define SHD __host__ __device__ __forceinline__
@@ -61,8 +63,17 @@ static inline SaTile sa_tile_make(int TX, int TY, int kChunk) {
 }
 // Thread tile and k chunk for nPlanes owned planes of block d on nSM multiprocessors with ctasPerSM resident CTAs each:
 // 32 x 4 or 16 x 8 (full 128-byte rows either way), whichever loads fewer halo cells over the block; then the longest
-// k chunk that still fills every resident CTA slot once.
+// k chunk that still fills every resident CTA slot once.  ADFB_SA_TILE=TX,TY,kChunk (tests) is taken instead when it fits
+// the shared buffers, the chunk clamped to nPlanes; one that does not fit leaves the pick to the chooser.
 static inline SaTile sa_tile_choose(const Dims& d, int nPlanes, int nSM, int ctasPerSM) {
+    if (const char* e = getenv("ADFB_SA_TILE")) {
+        int ox = 0, oy = 0, okc = 0;
+        sscanf(e, "%d,%d,%d", &ox, &oy, &okc);
+        if (ox >= 1 && oy >= 1 && ox <= SA_MAXT && oy <= SA_MAXT) {
+            const SaTile o = sa_tile_make(ox, oy, okc < nPlanes ? okc : nPlanes);
+            if (sa_tile_fits(o)) return o;
+        }
+    }
     const int shapes[2][2] = {{32, 4}, {16, 8}};
     long long best = -1;
     SaTile t = sa_tile_make(32, 4, 1);

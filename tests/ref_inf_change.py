@@ -21,6 +21,7 @@ computeEtotBlock(2, il, 2, jl, 2, kl) (haloExchange.F90:174-197), through the tr
 import ctypes as C
 import hashlib
 import os
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -124,16 +125,24 @@ def lib():
               os.path.join(REF, "src", "initFlow", "initializeFlow.F90"), os.path.join(REF, "src", "utils", "utils.F90"), _SO_BASE):
         with open(p, "rb") as f:
             h.update(f.read())
+    # the library is bound to this tree's libblockette_ref.so by its run path: a checkout elsewhere with the same sources
+    # must not load it, or the translation and the harness would each see their own copy of the module variables
+    h.update(os.path.abspath(_SO_BASE).encode())
     outdir = os.path.join(tempfile.gettempdir(), "adfb_ref_infchange_%d_%s" % (os.getuid(), h.hexdigest()[:12]))
     so = os.path.join(outdir, "libinfchange_ref.so")
     if not os.path.exists(so):
         os.makedirs(outdir, exist_ok=True)
-        srcs = _translate(outdir)
-        tmp = so + ".%d" % os.getpid()
-        subprocess.check_call(["gcc", "-O2", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-std=gnu11", "-w", "-shared",
-                               "-I" + _REFDIR, "-I" + os.path.join(ROOT, "oracle"), "-Wl,-Bsymbolic", "-o", tmp] + srcs
-                              + [_SO_BASE, "-Wl,-rpath," + _REFDIR, "-lm"])
-        os.replace(tmp, so)
+        # sources and library in a directory of this process's own: test processes running side by side may build at once
+        work = tempfile.mkdtemp(dir=outdir)
+        try:
+            srcs = _translate(work)
+            tmp = os.path.join(work, "libinfchange_ref.so")
+            subprocess.check_call(["gcc", "-O2", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-std=gnu11", "-w", "-shared",
+                                   "-I" + _REFDIR, "-I" + os.path.join(ROOT, "oracle"), "-Wl,-Bsymbolic", "-o", tmp] + srcs
+                                  + [_SO_BASE, "-Wl,-rpath," + _REFDIR, "-lm"])
+            os.replace(tmp, so)
+        finally:
+            shutil.rmtree(work, ignore_errors=True)
     _L = C.CDLL(so)
     return _L
 

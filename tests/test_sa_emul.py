@@ -12,6 +12,8 @@ import subprocess
 import numpy as np
 import pytest
 
+import sa_configs as SC
+from sa_configs import OPTIONS
 from util import FLOW, TURB, case, oracle_residual, rel_l2, rel_max
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -68,10 +70,6 @@ def test_emulated_sa_row_matches_oracle(shape, tile):
     prm, hb = case(*shape)
     ho = oracle_residual(prm, hb, FLOW | TURB)
     _check(hb, run_emul(prm, hb, *tile), ho.dw[..., 5])
-
-
-OPTIONS = [{"turbulenceOrder": "second order"}, {"turbulenceProduction": "vorticity"}, {"useRotationSA": True}, {"useft2SA": False},
-           {"useApproxSA": True}, {"turbulenceOrder": "second order", "turbulenceProduction": "vorticity", "useft2SA": False}]
 
 
 @pytest.mark.parametrize("opt", OPTIONS, ids=lambda o: "-".join("%s=%s" % kv for kv in o.items()))
@@ -141,3 +139,36 @@ def test_emulated_sa_row_in_low_reynolds_regime():
     ho = oracle_residual(prm, hb, FLOW | TURB)
     for tile in ((7, 4, 3), (16, 8, 1)):
         _check(hb, run_emul(prm, hb, *tile), ho.dw[..., 5])
+
+
+_ORACLE = {}
+
+
+def _oracle_row(shape):
+    if shape not in _ORACLE:
+        prm, hb = case(*shape)
+        _ORACLE[shape] = (prm, hb, oracle_residual(prm, hb, FLOW | TURB).dw[..., 5])
+    return _ORACLE[shape]
+
+
+@pytest.mark.parametrize("config", SC.CONFIGS, ids=SC.config_id)
+def test_emulated_sa_row_configurations(config):
+    """the configuration matrix tests/test_sa_tile_gpu.py runs on the device, with the same plane-by-plane comparison"""
+    shape, tile = config
+    prm, hb, want = _oracle_row(shape)
+    ow = hb.d.owned()
+    SC.assert_sa_planes(run_emul(prm, hb, *tile)[ow], want[ow])
+
+
+@pytest.mark.parametrize("shape,n_sm,ctas", [((96, 72, 64), 132, 3), ((128, 128, 64), 132, 3), ((160, 160, 144), 132, 3),
+                                             ((37, 13, 17), 132, 3), ((37, 13, 17), 1, 3), ((33, 9, 23), 5, 3),
+                                             ((24, 16, 12), 5, 2), ((129, 17, 16), 132, 3), ((96, 97, 9), 132, 3)])
+def test_restated_chooser_is_the_host_chooser(shape, n_sm, ctas):
+    """sa_configs.sa_tile_choose (which the device tests use to predict launches) is sa_tile_choose, and the bench picks
+    of sa_configs.BENCH_PICKS are what it gives"""
+    L = C.CDLL(_build())
+    out = (C.c_int * 4)()
+    assert L.emul_sa_choose(shape[0], shape[1], shape[2], shape[2], n_sm, ctas, out) == 0
+    assert tuple(out)[:3] == SC.sa_tile_choose(shape, shape[2], n_sm, ctas)
+    if shape in SC.BENCH_PICKS and (n_sm, ctas) == (SC.H100_SMS, SC.SA_CTAS_PER_SM):
+        assert tuple(out)[:3] == SC.BENCH_PICKS[shape]
