@@ -43,7 +43,7 @@ class AdfbSubface(C.Structure):
         ("ps", C.c_void_p), ("rho", C.c_void_p), ("velx", C.c_void_p), ("vely", C.c_void_p), ("velz", C.c_void_p),
         ("ptInlet", C.c_void_p), ("ttInlet", C.c_void_p), ("htInlet", C.c_void_p), ("flowXdirInlet", C.c_void_p),
         ("flowYdirInlet", C.c_void_p), ("flowZdirInlet", C.c_void_p), ("turbInlet", C.c_void_p),
-        ("subsonicInletTreatment", C.c_int32), ("pad_", C.c_int32),
+        ("subsonicInletTreatment", C.c_int32), ("pad_", C.c_int32), ("iblank", C.c_void_p),
     ]
 
 

@@ -639,6 +639,13 @@ int adfb_block_set_bc(int blk, int nSub, const AdfbSubface* subfaces) {
         if (up(sf.ps, 1) || up(sf.rho, 1) || up(sf.velx, 1) || up(sf.vely, 1) || up(sf.velz, 1) || up(sf.ptInlet, 1) || up(sf.ttInlet, 1) ||
             up(sf.htInlet, 1) || up(sf.flowXdirInlet, 1) || up(sf.flowYdirInlet, 1) || up(sf.flowZdirInlet, 1) || up(sf.turbInlet, 1))
             return 1;
+        if (sf.iblank) {
+            void* q = nullptr;
+            if (cudaMalloc(&q, n * sizeof(int32_t)) != cudaSuccess) return fail("adfb_block_set_bc: cudaMalloc failed");
+            b->bcAllocs.push_back(q);
+            if (cudaMemcpy(q, sf.iblank, n * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) return fail("adfb_block_set_bc: copy failed");
+            sf.iblank = (const int32_t*)q;
+        }
         if (sf.bcType == ADFB_BC_SUBSONIC_OUTFLOW && !sf.ps) return fail("adfb_block_set_bc: subsonic outflow needs ps");
         if (sf.bcType == ADFB_BC_SUPERSONIC_INFLOW && !(sf.ps && sf.rho && sf.velx && sf.vely && sf.velz))
             return fail("adfb_block_set_bc: supersonic inflow needs rho, velx, vely, velz, ps");

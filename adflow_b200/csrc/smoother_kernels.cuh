@@ -628,9 +628,10 @@ static int lines_per_cta(long long nLinesTotal, int n, int nArr, int maxLpc, siz
 
 // wallIntegrationFace, force and moment part (src/solver/surfaceIntegrations.F90:406-881): one CTA per wall
 // subface; every thread sums its face cells in index order, then a fixed-order tree reduction, so the result
-// is run-to-run reproducible.  acc = Fp(3), Fv(3), Mp(3), Mv(3).
-__global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev f, int dir, int isMin, int la, int lb, int viscWall,
-                                                     double r0, double r1, double r2, double pRef, double* acc) {
+// is run-to-run reproducible.  acc = Fp(3), Fv(3), Mp(3), Mv(3).  sib: the subface's surface iblank (BCData%iblank,
+// extents icBeg:icEnd x jcBeg:jcEnd), NULL == 1.
+__global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev f, const int32_t* sib, int dir, int isMin, int la, int lb,
+                                                     int viscWall, double r0, double r1, double r2, double pRef, double* acc) {
     ADFB_PDL_SYNC();
     __shared__ double sh[12][256];
     const long long N = d.N;
@@ -639,6 +640,7 @@ __global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev
     const int a0 = f.icBeg < 2 ? 2 : f.icBeg, a1 = f.icEnd > la ? la : f.icEnd;
     const int b0 = f.jcBeg < 2 ? 2 : f.jcBeg, b1 = f.jcEnd > lb ? lb : f.jcEnd;
     const int na = a1 - a0 + 1, nb = b1 - b0 + 1;
+    const int nfa = f.icEnd - f.icBeg + 1;
     const long long pstride = dir == 0 ? d.NJ : d.NI;
     const double* tau = b.wallTau + ((long long)(dir * 2 + (isMin ? 0 : 1)) * 9) * b.wallP;
     double v[12];
@@ -649,7 +651,7 @@ __global__ void __launch_bounds__(256) k_wall_forces(Dims d, BlockDev b, FaceDev
         const long long q = ia * f.sa + jb * f.sb;
         const long long c1 = f.off[1] + q, c2 = f.off[2] + q;
         const long long cf = isMin ? c1 : c2;
-        const double blk = dmax_((double)b.iblank[c2], 0.0);
+        const double blk = sib ? dmax_((double)sib[(ia - f.icBeg) + nfa * (jb - f.jcBeg)], 0.0) : 1.0;
         double xc[3];
 #pragma unroll
         for (int m = 0; m < 3; m++) {
@@ -862,7 +864,7 @@ static int launch_wall_forces(const Dims& d, const BlockDev& b, const std::vecto
         const int dir = (sf.faceId - 1) / 2, isMin = (sf.faceId % 2) == 1;
         const int la = dir == 0 ? d.jl : d.il, lb = dir == 2 ? d.jl : d.kl;
         KT_BEGIN(K_MISC, s);
-        launch_pdl(k_wall_forces, 1, 256, s, d, b, f, dir, isMin, la, lb, viscWall ? 1 : 0, rp[0], rp[1], rp[2], pRef, acc);
+        launch_pdl(k_wall_forces, 1, 256, s, d, b, f, sf.iblank, dir, isMin, la, lb, viscWall ? 1 : 0, rp[0], rp[1], rp[2], pRef, acc);
         KT_END(K_MISC, s);
     }
     return (int)cudaGetLastError();

@@ -70,6 +70,12 @@ class ADFLOW_B200:
                     a = np.asfortranarray(a, dtype=np.float64)
                     keep.append(a)
                     setattr(sf[q], name, a.ctypes.data)
+            if s.get("iblank") is not None:   # BCData%iblank, int32 (icBeg:icEnd, jcBeg:jcEnd)
+                a = np.asfortranarray(s["iblank"], dtype=np.int32)
+                if a.shape != (s["icEnd"] - s["icBeg"] + 1, s["jcEnd"] - s["jcBeg"] + 1):
+                    raise ValueError("subface %d: iblank has shape %s, not the subface's cell range" % (q, a.shape))
+                keep.append(a)
+                sf[q].iblank = a.ctypes.data
         check(self.L.adfb_block_set_bc(blk, n, sf), "adfb_block_set_bc")
 
     def uploadState(self, blk, hb, with_visc=True):

@@ -226,11 +226,12 @@ def make_block(nx, ny, nz, prm, origin=(0, 0, 0), global_n=None, first_cell="aut
     return blk
 
 
-def make_subface(blk, face, bc, prm=None):
+def make_subface(blk, face, bc, prm=None, iblank=None):
     """BCData of one whole block face: cell range 1:ie x 1:je of the two in-plane
     directions (halo-extended like icBeg:icEnd, src/utils/utils.F90:895-900) and the
     unit outward normal from the face's s-vector (boundaryNormals,
-    src/adjoint/adjointExtra.F90)."""
+    src/adjoint/adjointExtra.F90).  iblank: the surface blanking BCData%iblank over that
+    range (key "iblank"); absent means 1 everywhere."""
     d = blk.d
     if face in (IMIN, IMAX):
         n1, n2 = d.je, d.ke
@@ -247,6 +248,9 @@ def make_subface(blk, face, bc, prm=None):
     mag = np.where(mag > 0, mag, 1.0)
     norm = np.asfortranarray(mult * s / mag[..., None])
     sub = {"bcType": bc, "faceId": face, "icBeg": 1, "icEnd": n1, "jcBeg": 1, "jcEnd": n2, "norm": norm}
+    if iblank is not None:
+        assert np.shape(iblank) == (n1, n2), np.shape(iblank)
+        sub["iblank"] = np.asfortranarray(iblank, dtype=np.int32)
     a, c = np.meshgrid(np.arange(n1), np.arange(n2), indexing="ij")
     wig = np.sin(0.37 * a) * np.cos(0.23 * c)          # smooth in-plane variation of the prescribed data
     if bc == 6:  # isothermal wall: BCData%TNS_Wall, non-dimensional (T_inf = 1), smooth 5 % variation

@@ -163,6 +163,11 @@ typedef struct AdfbSubface {
     const double* turbInlet;                /* BCData%turbInlet(:,:,nt1:nt2): turbulence variable at inflow faces */
     int32_t subsonicInletTreatment;         /* 1 totalConditions, 2 massFlow (constants.F90:237-238) */
     int32_t pad_;
+    /* BCData%iBlank (BCData.F90:2176), extents (icBeg:icEnd, jcBeg:jcEnd): the surface blanking of the face cells that
+       weights them in adfb_forces.  NULL == 1 everywhere, the reference's value without overset (BCData.F90:2182).  With
+       overset the zipper derives it from the first cell layer's iblank and then changes it (zipperMesh.F90:795-829,
+       955-989, 1510-1567, 352-376), so it is not the volume iblank of the adjacent cell. */
+    const int32_t* iblank;
 } AdfbSubface;
 
 /* ---- life cycle ---------------------------------------------------------- */
@@ -256,7 +261,9 @@ int adfb_synchronize(void);
 /* wallIntegrationFace / getForces (src/solver/surfaceIntegrations.F90:406-881, src/warping/getForces.F90):
    out = Fp(3), Fv(3), Mp(3), Mv(3) summed over the wall subfaces (viscous walls: pressure + viscous, Euler walls:
    pressure) of all blocks of `level` on all ranks; moments about refPoint; forces scaled by pRef like the
-   reference.  The viscous part needs a preceding adfb_residual(level, flags | ADFB_RES_STORE_WALL). */
+   reference.  Each face cell is weighted by max(surface iblank, 0), the AdfbSubface.iblank of its subface
+   (BCData%iblank, surfaceIntegrations.F90:538, 716), not by the iblank of the adjacent interior cell.  The viscous part
+   needs a preceding adfb_residual(level, flags | ADFB_RES_STORE_WALL). */
 int adfb_forces(int level, const double refPoint[3], double pRef, double out[12]);
 
 /* referenceShockSensor (src/adjoint/adjointUtils.F90:1900-1950): freeze the shock sensor

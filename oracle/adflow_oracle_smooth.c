@@ -754,8 +754,13 @@ void orc_dadi_step(const OrcBlock* b, const AdfbParams* prm0, int nSub, const Ad
 /* ------------------------------------------------------------------------ */
 /* wallIntegrationFace, src/solver/surfaceIntegrations.F90:406-881: pressure and viscous force / moment sums of
    the wall subfaces.  BCPointers planes (setBCPointers with spatialPointers): pp2 / pp1 = first interior / first
-   halo pressure, ssi = face normal of the wall face, xx = its node coordinates, fact = -1 on min faces.
+   halo pressure, ssi = face normal of the wall face, xx = its node coordinates, fact = -1 on min faces.  Face cells are
+   weighted by max(BCData%iblank, 0) of the subface (sf->iblank, NULL == 1), not by the volume iblank.
    Owned face cells only (inBeg+1:inEnd): 2..l of the two in-plane directions. */
+static double surface_blank(const AdfbSubface* sf, int ia, int jb) {
+    if (!sf->iblank) return one;
+    return dmax((double)sf->iblank[(ia - sf->icBeg) + (sf->icEnd - sf->icBeg + 1) * (jb - sf->jcBeg)], zero);
+}
 void orc_wall_forces(const OrcBlock* b, const AdfbParams* prm, int nSub, const AdfbSubface* sfs, const double refPoint[3],
                      double pRef, double out[12]) {
     Dims d = dims_of(b);
@@ -784,7 +789,7 @@ void orc_wall_forces(const OrcBlock* b, const AdfbParams* prm, int nSub, const A
             double xc[3];
             for (int m = 0; m < 3; m++)
                 xc[m] = fourth * (X(cf - f.sa - f.sb, m) + X(cf - f.sb, m) + X(cf - f.sa, m) + X(cf, m));
-            double blk = dmax((double)b->iblank[c2], zero);
+            double blk = surface_blank(sf, ia, jb_);
             double fx = pm1 * s[cf], fy = pm1 * s[d.N + cf], fz = pm1 * s[2 * d.N + cf];
             double rx = xc[0] - refPoint[0], ry = xc[1] - refPoint[1], rz = xc[2] - refPoint[2];
             Fp[0] += fx * blk; Fp[1] += fy * blk; Fp[2] += fz * blk;
@@ -796,7 +801,7 @@ void orc_wall_forces(const OrcBlock* b, const AdfbParams* prm, int nSub, const A
                 long q = ia * f.sa + jb_ * f.sb;
                 long c1 = f.off[1] + q, c2 = f.off[2] + q;
                 long cf = isMin ? c1 : c2;
-                double blk = dmax((double)b->iblank[c2], zero);
+                double blk = surface_blank(sf, ia, jb_);
                 double txx = t[cf], tyy = t[d.N + cf], tzz = t[2 * d.N + cf], txy = t[3 * d.N + cf], txz = t[4 * d.N + cf],
                        tyz = t[5 * d.N + cf];
                 double s1 = s[cf], s2 = s[d.N + cf], s3 = s[2 * d.N + cf];

@@ -118,6 +118,10 @@ class Oracle:
                     a = np.asfortranarray(a, dtype=np.float64)
                     self._keep.append(a)
                     setattr(arr[q], name, a.ctypes.data)
+            if s.get("iblank") is not None:   # BCData%iblank, int32 (icBeg:icEnd, jcBeg:jcEnd)
+                a = np.asfortranarray(s["iblank"], dtype=np.int32)
+                self._keep.append(a)
+                arr[q].iblank = a.ctypes.data
         return len(subs), arr
 
     def apply_turb_bc(self, second_halo=True):

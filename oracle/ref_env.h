@@ -77,7 +77,7 @@ typedef struct {
     int icbeg, icend, jcbeg, jcend;
     double *norm, *rface, *uslip, *tns_wall;
     int inbeg, inend, jnbeg, jnend; /* node range of the subface (owned face cells are inBeg+1:inEnd) */
-    int* iblank;                    /* BCData%iblank: iblank of the adjacent interior cell, (icBeg:icEnd, jcBeg:jcEnd) */
+    int* iblank;                    /* BCData%iblank: surface blanking of the face cells, (icBeg:icEnd, jcBeg:jcEnd) */
     double* tau;                    /* viscSubface%tau(:,:,6), same layout */
     /* in/outflow data */
     double *ps, *rho, *velx, *vely, *velz, *ptinlet, *ttinlet, *htinlet, *flowxdirinlet, *flowydirinlet, *flowzdirinlet, *turbinlet;

@@ -171,7 +171,6 @@ def bind_bcs(hb, prm, other_level=False):
         tab[q].inbeg, tab[q].inend = max(s_["icBeg"], 2) - 1, min(s_["icEnd"], la)
         tab[q].jnbeg, tab[q].jnend = max(s_["jcBeg"], 2) - 1, min(s_["jcEnd"], lb)
         ra, rb = slice(s_["icBeg"], s_["icEnd"] + 1), slice(s_["jcBeg"], s_["jcEnd"] + 1)
-        inner = {1: 2, 2: d.il, 3: 2, 4: d.jl, 5: 2, 6: d.kl}[face]       # first interior cell plane
         fplane = {1: 1, 2: d.il, 3: 1, 4: d.jl, 5: 1, 6: d.kl}[face]      # index of the boundary face
         ax = (face - 1) // 2
 
@@ -180,7 +179,10 @@ def bind_bcs(hb, prm, other_level=False):
             sl.insert(ax, idx)
             return arr[tuple(sl)]
 
-        ib_ = np.asfortranarray(plane(hb.iblank, inner).astype(np.int32))
+        # BCData%iblank: the subface's own surface blanking, 1 where the host gives none (BCData.F90:2182)
+        ib_ = s_.get("iblank")
+        ib_ = np.ones((na, nb), dtype=np.int32, order="F") if ib_ is None else np.asfortranarray(ib_, dtype=np.int32)
+        assert ib_.shape == (na, nb), ib_.shape
         keep.append(ib_)
         tab[q].iblank = ib_.ctypes.data
         tau = np.asfortranarray(plane(hb.wallTau, fplane)[..., 9 * ax:9 * ax + 6].astype(np.float64))
