@@ -17,7 +17,7 @@ ABI_SYMBOLS = [
     "adfb_init", "adfb_finalize", "adfb_get_unique_id", "adfb_last_error", "adfb_device_count",
     "adfb_block_create", "adfb_block_destroy", "adfb_block_set_geometry", "adfb_block_set_bc",
     "adfb_set_params", "adfb_upload_state", "adfb_download_state", "adfb_upload_visc",
-    "adfb_download_residual", "adfb_download_intermed", "adfb_residual", "adfb_norms", "adfb_synchronize", "adfb_forces",
+    "adfb_download_residual", "adfb_download_intermed", "adfb_residual", "adfb_norms", "adfb_monitor", "adfb_synchronize", "adfb_forces",
     "adfb_set_total_residuals", "adfb_free_stream_residual", "adfb_inf_change_correction", "adfb_set_uniform_flow",
     "adfb_get_states", "adfb_set_states", "adfb_get_res", "adfb_state_size",
     "adfb_comm_set_pattern", "adfb_comm_set_overset", "adfb_block_set_orphans", "adfb_halo_exchange",
@@ -78,6 +78,7 @@ def load():
     L.adfb_download_array.argtypes = [ci, C.c_char_p, vp]
     L.adfb_residual.argtypes = [ci, cu]
     L.adfb_norms.argtypes = [C.POINTER(C.c_double)]
+    L.adfb_monitor.argtypes = [ci, cu, C.POINTER(C.c_double)]
     L.adfb_set_total_residuals.argtypes = [C.c_double, C.c_double]
     L.adfb_free_stream_residual.argtypes = [C.POINTER(C.c_double)]
     L.adfb_inf_change_correction.argtypes = [C.POINTER(C.c_double), C.c_double, ci, C.POINTER(ci)]

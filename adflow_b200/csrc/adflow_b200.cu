@@ -67,6 +67,8 @@ struct Context {
     std::vector<Block> blocks;
     double* dRed = nullptr;   // reduction scratch
     size_t dRedN = 0;
+    double* dMon = nullptr;   // monitor partials, one slot per block of the level, and the results
+    size_t dMonN = 0;
     double* hRed = nullptr;   // pinned
     double* dVec = nullptr;   // AoS staging vector (get/set states, get res)
     size_t dVecN = 0;
@@ -429,6 +431,8 @@ int adfb_finalize(void) {
     g.blocks.clear();
     if (g.dRed) cudaFree(g.dRed);
     g.dRed = nullptr; g.dRedN = 0;
+    if (g.dMon) cudaFree(g.dMon);
+    g.dMon = nullptr; g.dMonN = 0;
     if (g.dMffd) { cudaFree(g.dMffd); g.dMffd = nullptr; }
     if (g.hMffd) { cudaFreeHost(g.hMffd); g.hMffd = nullptr; }
     if (g.dVec) cudaFree(g.dVec);
@@ -2432,34 +2436,66 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
     return 0;
 }
 
+// The monitor values of the live blocks of `level` (layout of adfb_monitor): every block's partials in a slot of its
+// own, one CTA combining them in block-id order, the sums and the maxima all-reduced, one synchronisation.  No block:
+// zeros (this rank still joins the all-reductions).
+static int monitor_impl(int level, unsigned what, double out[ADFB_MON_N]) {
+    const int nPart = 1024;   // fixed partition: adfb_norms has summed each block over 1024 x 256 threads from the start
+    const long long stride = (long long)ADFB_MON_N * nPart;
+    int nBlk = 0;
+    for (const Block& b : g.blocks) nBlk += b.alive && b.level == level;
+    const size_t need = (size_t)std::max(nBlk, 1) * stride + ADFB_MON_N;
+    if (g.dMonN < need) {
+        if (g.dMon) cudaFree(g.dMon);
+        g.dMon = nullptr; g.dMonN = 0;
+        CK(cudaMalloc((void**)&g.dMon, need * sizeof(double)));
+        g.dMonN = need;
+    }
+    double* res = g.dMon + (size_t)std::max(nBlk, 1) * stride;
+    MonCoef mc = {};
+    mc.turbResScale = g.prm.turbResScale;
+    mc.hInf = (g.prm.wInf[4] + g.prm.pInfCorr) / g.prm.rhoInf;
+    mc.gamma = g.prm.gammaInf;
+    mc.eddy = g.prm.equations == ADFB_RANS;
+    int bi = 0;
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != level) continue;
+        mc.nw = b.nw;
+        if (launch_norms_partial(b.d, b.dev, mc, what, g.dMon + bi * stride, nPart, g.stream)) return fail("monitor kernel failed");
+        bi++;
+    }
+    if (launch_norms_final(g.dMon, nPart, stride, nBlk, what, mc.hInf, res, g.stream)) return fail("monitor kernel failed");
+    if (g.nranks > 1) {   // mpi_allreduce of monLoc: the sums with mpi_sum, the maxima with mpi_max (solvers.F90:1537-1545)
+        int rc = g.nccl.AllReduce(res, res, ADFB_MON_NSUM, kNcclDouble, kNcclSum, g.comm, g.stream);
+        if (rc == 0) rc = g.nccl.AllReduce(res + ADFB_MON_NSUM, res + ADFB_MON_NSUM, ADFB_MON_N - ADFB_MON_NSUM, kNcclDouble, kNcclMax, g.comm, g.stream);
+        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
+    }
+    CK(cudaMemcpyAsync(g.hRed, res, ADFB_MON_N * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
+    CK(cudaStreamSynchronize(g.stream));
+    for (int v = 0; v < ADFB_MON_N; v++) out[v] = g.hRed[v];
+    return 0;
+}
+
+int adfb_monitor(int level, unsigned what, double out[10]) {
+    ADFB_RANGE("adfb_monitor");
+    NEED_INIT();
+    if (!out) return fail("adfb_monitor: null");
+    if (what == 0 || (what & ~3u)) return fail("adfb_monitor: what must be 1 (sums), 2 (maxima) or 3 (both), got %u", what);
+    if (!g.havePrm) return fail("adfb_monitor: adfb_set_params has not been called");
+    bool have = false;
+    for (const Block& b : g.blocks) have = have || (b.alive && b.level == level);
+    if (!have) return fail("adfb_monitor: no block of level %d", level);
+    return monitor_impl(level, what, out);
+}
+
 int adfb_norms(double out[2]) {
     ADFB_RANGE("adfb_norms");
     NEED_INIT();
     if (!out) return fail("adfb_norms: null");
-    out[0] = out[1] = 0.0;
-    for (Block& b : g.blocks) {
-        if (!b.alive || b.level != 1) continue;
-        const int nPart = 1024;
-        if (g.dRedN < (size_t)2 * nPart + 2) {
-            if (g.dRed) cudaFree(g.dRed);
-            CK(cudaMalloc((void**)&g.dRed, (2 * nPart + 2) * sizeof(double)));
-            g.dRedN = 2 * nPart + 2;
-        }
-        if (launch_norms(b.d, b.dev, b.nw, g.prm.turbResScale, g.dRed, nPart, g.stream)) return fail("norm kernel failed");
-        CK(cudaMemcpyAsync(g.hRed, g.dRed + 2 * nPart, 2 * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-        CK(cudaStreamSynchronize(g.stream));
-        out[0] += g.hRed[0];
-        out[1] += g.hRed[1];
-    }
-    if (g.nranks > 1) {  // mpi_allreduce(monLoc, monGlob, ...), NKSolvers.F90:364
-        g.hRed[0] = out[0]; g.hRed[1] = out[1];
-        CK(cudaMemcpyAsync(g.dRed, g.hRed, 2 * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-        const int rc = g.nccl.AllReduce(g.dRed, g.dRed, 2, kNcclDouble, kNcclSum, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-        CK(cudaMemcpyAsync(g.hRed, g.dRed, 2 * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-        CK(cudaStreamSynchronize(g.stream));
-        out[0] = g.hRed[0]; out[1] = g.hRed[1];
-    }
+    double m[ADFB_MON_N];
+    if (monitor_impl(1, 1, m)) return 1;
+    out[0] = m[0];
+    out[1] = m[6];
     return 0;
 }
 

@@ -170,4 +170,5 @@ struct NcclApi {
 };
 static const int kNcclDouble = 8;  // ncclFloat64 (nccl.h ncclDataType_t)
 static const int kNcclSum = 0;     // ncclSum
+static const int kNcclMax = 2;     // ncclMax
 static const int kNcclMin = 3;     // ncclMin (nccl.h ncclRedOp_t: sum, prod, max, min)

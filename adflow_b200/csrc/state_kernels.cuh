@@ -5,7 +5,8 @@
 //   k_state_prep : computePressureSimple (src/utils/flowUtils.F90:867-930),
 //                  computeLamViscosity (:1201-1323), saEddyViscosity
 //                  (src/turbulence/turbUtils.F90:657-712) fused in one pass
-//   k_norms      : sumResiduals / sumAllResiduals (src/utils/utils.F90:6364-6459)
+//   k_norms      : sumResiduals / sumAllResiduals (src/utils/utils.F90:6364-6459), maxHdiffMach / maxEddyv
+//                  (:2422-2531): the convergence monitor of adfb_monitor and adfb_norms
 #pragma once
 #include <limits.h>
 #include "adfb_common.cuh"
@@ -103,44 +104,114 @@ __global__ void __launch_bounds__(256) k_etot_owned(Dims d, BlockDev b) {
     b.w[4 * N + c] = c_fheat[7] /* 1/(gamma-1) */ * b.p[c] + 0.5 * r * (u * u + v * v + w * w);
 }
 
-// two-pass deterministic reduction: pass 1 -> nPart partial pairs, pass 2 -> final pair
-__global__ void __launch_bounds__(256) k_norms_partial(Dims d, BlockDev b, int nw, double turbResScale, double* part, int nPart) {
-    __shared__ double s0[256], s1[256];
+// The monitor values of convergenceInfo (solvers.F90:1338-1376) over the owned cells 2:il, 2:jl, 2:kl of one block, in
+// the layout of adfb_monitor: 0..5 sumResiduals (utils.F90:6364-6398) of rho, rho u, rho v, rho w, rho E, nu~;
+// 6 sumAllResiduals (:6400-6448); 7 max |(rhoE + p) / rho - hInf| and 8 max Mach^2 of maxHdiffMach (:2466-2531), before
+// its division by hInf and square root; 9 max rev / rlv of maxEddyv (:2422-2464).
+enum { ADFB_MON_N = 10, ADFB_MON_NSUM = 7 };
+struct MonCoef {
+    double turbResScale, hInf, gamma;
+    int nw, eddy;   // eddy: an eddy-viscosity model (RANS), else maxEddyv is 0
+};
+
+// Two-pass deterministic reduction.  Pass 1, per block: CTA q of nPart writes its partial of value v to part[v nPart + q];
+// a grid-stride loop of a fixed grid, then a fixed tree.  what: bit 0 the sums, bit 1 the maxima; a cleared bit skips
+// the work and the loads behind it, and its partials are not written.  The maxima form each cell's value with explicit
+// roundings (no FMA contraction), so they are the reference's bits; fmax ignores a NaN operand, so a NaN cell does not
+// enter them.
+__global__ void __launch_bounds__(256) k_norms_partial(Dims d, BlockDev b, MonCoef mc, unsigned what, double* part, int nPart) {
+    __shared__ double s[ADFB_MON_N][256];
     const long long nOwned = (long long)d.nx * d.ny * d.nz;
-    double a0 = 0.0, a1 = 0.0;
+    const bool sums = what & 1, maxima = what & 2;
+    const int v0 = sums ? 0 : ADFB_MON_NSUM, v1 = maxima ? ADFB_MON_N : ADFB_MON_NSUM;
+    double a[ADFB_MON_N];
+#pragma unroll
+    for (int v = 0; v < ADFB_MON_N; v++) a[v] = 0.0;
     const long long N = d.N;
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < nOwned; q += (long long)gridDim.x * blockDim.x) {
         const int i = (int)(q % d.nx) + 2;
         const int j = (int)((q / d.nx) % d.ny) + 2;
         const int k = (int)(q / ((long long)d.nx * d.ny)) + 2;
         const long long c = ADFB_IDX(i, j, k);
-        const double ovv = 1.0 / b.vol[c];
-        const double r = b.dw[c] / b.vol[c];
-        a0 += r * r;
-        double ssum = 0.0;
-        for (int l = 0; l < 5; l++) { const double t = b.dw[l * N + c] * ovv; ssum += t * t; }
-        for (int l = 5; l < nw; l++) { const double t = b.dw[l * N + c] * ovv * turbResScale; ssum += t * t; }
-        a1 += ssum;
+        if (sums) {
+            const double vol = b.vol[c];
+            const double ovv = 1.0 / vol;
+            double ssum = 0.0;   // state_sum: the cell's terms in variable order, then added to the total
+#pragma unroll
+            for (int l = 0; l < 5; l++) {
+                const double dw = b.dw[l * N + c];
+                const double r = dw / vol;
+                a[l] += r * r;
+                const double t = dw * ovv;
+                ssum += t * t;
+            }
+            for (int l = 5; l < mc.nw; l++) {
+                const double dw = b.dw[l * N + c];
+                const double r = dw / vol;
+                a[5] += r * r;
+                const double t = dw * ovv * mc.turbResScale;
+                ssum += t * t;
+            }
+            a[6] += ssum;
+        }
+        if (maxima) {
+            const double rho = b.w[c], u = b.w[N + c], v = b.w[2 * N + c], w = b.w[3 * N + c], p = b.p[c];
+            const double hdiff = fabs(__dsub_rn(__ddiv_rn(__dadd_rn(b.w[4 * N + c], p), rho), mc.hInf));
+            const double v2 = __dadd_rn(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v)), __dmul_rn(w, w));
+            const double mach2 = __ddiv_rn(__dmul_rn(v2, rho), __dmul_rn(mc.gamma, p));
+            a[7] = fmax(a[7], hdiff);
+            a[8] = fmax(a[8], mach2);
+            if (mc.eddy) a[9] = fmax(a[9], __ddiv_rn(b.rev[c], b.rlv[c]));
+        }
     }
-    s0[threadIdx.x] = a0; s1[threadIdx.x] = a1;
+#pragma unroll
+    for (int v = 0; v < ADFB_MON_N; v++) s[v][threadIdx.x] = a[v];
     __syncthreads();
     for (int st = 128; st > 0; st >>= 1) {
-        if ((int)threadIdx.x < st) { s0[threadIdx.x] += s0[threadIdx.x + st]; s1[threadIdx.x] += s1[threadIdx.x + st]; }
+        if ((int)threadIdx.x < st)
+            for (int v = v0; v < v1; v++) {
+                if (v < ADFB_MON_NSUM) s[v][threadIdx.x] += s[v][threadIdx.x + st];
+                else s[v][threadIdx.x] = fmax(s[v][threadIdx.x], s[v][threadIdx.x + st]);
+            }
         __syncthreads();
     }
-    if (threadIdx.x == 0) { part[blockIdx.x] = s0[0]; part[nPart + blockIdx.x] = s1[0]; }
+    if ((int)threadIdx.x >= v0 && (int)threadIdx.x < v1) part[threadIdx.x * nPart + blockIdx.x] = s[threadIdx.x][0];
 }
-__global__ void __launch_bounds__(256) k_norms_final(double* part, int nPart) {
-    __shared__ double s0[256], s1[256];
-    double a0 = 0.0, a1 = 0.0;
-    for (int q = threadIdx.x; q < nPart; q += 256) { a0 += part[q]; a1 += part[nPart + q]; }
-    s0[threadIdx.x] = a0; s1[threadIdx.x] = a1;
-    __syncthreads();
-    for (int st = 128; st > 0; st >>= 1) {
-        if ((int)threadIdx.x < st) { s0[threadIdx.x] += s0[threadIdx.x + st]; s1[threadIdx.x] += s1[threadIdx.x + st]; }
+
+// Pass 2, one CTA: block bi's partials at part + bi stride reduced by a fixed tree, then the blocks combined in block
+// order, sum = ((0 + b0) + b1) + ..., max from 0; out[7] / hInf and sqrt(out[8]) as maxHdiffMach ends (monotone, so
+// they commute with the maximum over blocks and ranks).  Entries of a cleared `what` bit are 0.
+__global__ void __launch_bounds__(256) k_norms_final(const double* __restrict__ part, int nPart, long long stride, int nBlk,
+                                                     unsigned what, double hInf, double* __restrict__ out) {
+    __shared__ double s[ADFB_MON_N][256];
+    __shared__ double tot[ADFB_MON_N];
+    if (threadIdx.x < ADFB_MON_N) tot[threadIdx.x] = 0.0;
+    const int v0 = (what & 1) ? 0 : ADFB_MON_NSUM, v1 = (what & 2) ? ADFB_MON_N : ADFB_MON_NSUM;
+    for (int bi = 0; bi < nBlk; bi++) {
+        const double* pb = part + bi * stride;
+        for (int v = v0; v < v1; v++) {
+            double a = 0.0;
+            if (v < ADFB_MON_NSUM) for (int q = threadIdx.x; q < nPart; q += 256) a += pb[v * nPart + q];
+            else for (int q = threadIdx.x; q < nPart; q += 256) a = fmax(a, pb[v * nPart + q]);
+            s[v][threadIdx.x] = a;
+        }
+        __syncthreads();
+        for (int st = 128; st > 0; st >>= 1) {
+            if ((int)threadIdx.x < st)
+                for (int v = v0; v < v1; v++) {
+                    if (v < ADFB_MON_NSUM) s[v][threadIdx.x] += s[v][threadIdx.x + st];
+                    else s[v][threadIdx.x] = fmax(s[v][threadIdx.x], s[v][threadIdx.x + st]);
+                }
+            __syncthreads();
+        }
+        if (threadIdx.x == 0)
+            for (int v = v0; v < v1; v++) tot[v] = v < ADFB_MON_NSUM ? tot[v] + s[v][0] : fmax(tot[v], s[v][0]);
         __syncthreads();
     }
-    if (threadIdx.x == 0) { part[2 * nPart] = s0[0]; part[2 * nPart + 1] = s1[0]; }
+    if (threadIdx.x == 0) {
+        if (what & 2) { tot[7] = __ddiv_rn(tot[7], hInf); tot[8] = __dsqrt_rn(tot[8]); }
+        for (int v = 0; v < ADFB_MON_N; v++) out[v] = tot[v];
+    }
 }
 
 // The per-call coefficients of the whole-state modes of k_vec, formed on the host: the free-stream change and the rotation
@@ -335,13 +406,18 @@ static int launch_state_prep(const Dims& d, const BlockDev& b, const AdfbParams&
     return (int)cudaGetLastError();
 }
 
-static int launch_norms(const Dims& d, const BlockDev& b, int nw, double turbResScale, double* part, int nPart,
-                        cudaStream_t stream) {
+// pass 1 of the monitor reduction on one block, into its own nPart x ADFB_MON_N slot of the partials
+static int launch_norms_partial(const Dims& d, const BlockDev& b, const MonCoef& mc, unsigned what, double* part, int nPart,
+                                cudaStream_t stream) {
     KT_BEGIN(K_NORMS, stream);
-    k_norms_partial<<<nPart, 256, 0, stream>>>(d, b, nw, turbResScale, part, nPart);
+    k_norms_partial<<<nPart, 256, 0, stream>>>(d, b, mc, what, part, nPart);
     KT_END(K_NORMS, stream);
+    return (int)cudaGetLastError();
+}
+static int launch_norms_final(const double* part, int nPart, long long stride, int nBlk, unsigned what, double hInf, double* out,
+                              cudaStream_t stream) {
     KT_BEGIN(K_NORMS, stream);
-    k_norms_final<<<1, 256, 0, stream>>>(part, nPart);
+    k_norms_final<<<1, 256, 0, stream>>>(part, nPart, stride, nBlk, what, hInf, out);
     KT_END(K_NORMS, stream);
     return (int)cudaGetLastError();
 }

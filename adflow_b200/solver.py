@@ -12,6 +12,8 @@ State/residual vectors use the reference ordering (``NKSolvers.F90:1240-1255``):
 for each block, k, j, i, then the nw variables of the cell (AoS per cell).
 """
 import ctypes as C
+import math
+import time
 
 import numpy as np
 
@@ -21,15 +23,77 @@ from ._lib import AdfbSubface, check, ptr
 RES_DISS_APPROX, RES_VISC_APPROX, RES_UPDATE_INTERMED = 1, 2, 4
 RES_FLOW, RES_TURB, RES_STORE_WALL, RES_SKIP_PREAMBLE = 8, 16, 32, 64
 
+# adfb_monitor: `what` bits and the entries of its out[10]
+MON_SUMS, MON_MAXIMA = 1, 2
+# the monitored quantities of convergenceInfo by their CGNS names (cgnsNames.f90), in the order checkMonitor sorts them
+# (inputParamRoutines.F90:120-330), with their entry of adfb_monitor's out[]
+MONITOR_SLOTS = {"RSDMassRMS": 0, "RSDMomentumXRMS": 1, "RSDMomentumYRMS": 2, "RSDMomentumZRMS": 3,
+                 "RSDEnergyStagnationDensityRMS": 4, "RSDTurbulentSANuTildeRMS": 5, "totalR": 6, "MaxDiffHAndHinf": 7,
+                 "MaxMach": 8, "MaxRatioEddyAndLaminarViscosity": 9}
+# the keywords of the pyADflow option monitorVariables (monitorVariables, inputParamRoutines.F90:1480-1660)
+_MONITOR_KEYWORDS = {"resrho": ["RSDMassRMS"], "resmom": ["RSDMomentumXRMS", "RSDMomentumYRMS", "RSDMomentumZRMS"],
+                     "resrhoe": ["RSDEnergyStagnationDensityRMS"], "resturb": ["RSDTurbulentSANuTildeRMS"],
+                     "totalr": ["totalR"], "hdiff": ["MaxDiffHAndHinf"], "mach": ["MaxMach"],
+                     "eddyv": ["MaxRatioEddyAndLaminarViscosity"]}
+_FORCE_MONITORS = ("cl", "clp", "clv", "cd", "cdp", "cdv", "cfx", "cfy", "cfz", "cmx", "cmy", "cmz")
+_SOLUTION_MONITORS = ("yplus", "sepsensor", "sepsensorksarea", "cavitation", "axismoment")
+# pyADflow's default monitorVariables without the force monitors cl and cd, which the device does not monitor
+DEFAULT_MONITOR_VARIABLES = ("cpu", "resrho", "resturb")
+
+
+def monitor_names(variables, rans):
+    """The CGNS names convergenceInfo monitors for the monitorVariables keywords `variables`, in its order, and whether
+    "cpu" (the host wall time) was asked for.  resrho and totalR are always monitored; resturb and eddyv only with RANS
+    (checkMonitor drops them otherwise).  The force and getSolution monitors are refused with a ValueError."""
+    names, cpu = {"RSDMassRMS", "totalR"}, False
+    for v in variables:
+        key = v.lower()
+        if key == "cpu":
+            cpu = True
+        elif key in _FORCE_MONITORS:
+            raise ValueError("monitor variable %r is a force or moment coefficient, which the device does not monitor: "
+                             "evaluate it with evalFunctions after residual(... | RES_STORE_WALL)" % v)
+        elif key in _SOLUTION_MONITORS:
+            raise ValueError("monitor variable %r is a getSolution quantity, which the device does not evaluate" % v)
+        elif key not in _MONITOR_KEYWORDS:
+            raise ValueError("unknown monitor variable %r; known: cpu, %s" % (v, ", ".join(sorted(_MONITOR_KEYWORDS))))
+        elif rans or key not in ("resturb", "eddyv"):
+            names.update(_MONITOR_KEYWORDS[key])
+    return [n for n in MONITOR_SLOTS if n in names], cpu
+
+
+def convergence_status(ground_level, approx_total_its, n_cycles, values, rho_res, rho_res_start, total_r, total_r0,
+                       total_r_start, L2Convergence=1e-8, L2ConvergenceCoarse=1e-2, L2ConvergenceRel=1e-16,
+                       maxL2DeviationFactor=1.0):
+    """(converged, failed) after one convergenceInfo of the steady solveState (solvers.F90:1726-1763, 1873-1920): above
+    ground level 1 rhoRes < L2ConvergenceCoarse rhoResStart; on level 1 totalR < L2Convergence totalR0 or
+    totalR < L2ConvergenceRel totalRStart.  Failed: a NaN among the monitored `values`, or on ground level 1 with the
+    nCycles cycles spent, totalR > maxL2DeviationFactor totalR0 L2Convergence."""
+    if ground_level != 1:
+        converged = rho_res < L2ConvergenceCoarse * rho_res_start
+    else:
+        converged = total_r < L2Convergence * total_r0 or total_r < L2ConvergenceRel * total_r_start
+    failed = any(math.isnan(v) for v in values)
+    if not failed and ground_level == 1 and approx_total_its >= n_cycles:
+        failed = total_r > maxL2DeviationFactor * total_r0 * L2Convergence
+    return bool(converged), bool(failed)
+
 
 class ADFLOW_B200:
     def __init__(self, prm, device=0, rank=0, nranks=1, unique_id=None):
         self.L = _lib.load()
         check(self.L.adfb_init(device, unique_id, rank, nranks), "adfb_init")
         self.prm = prm
+        self.nranks = nranks
         check(self.L.adfb_set_params(C.byref(prm)), "adfb_set_params")
         self.blocks = []  # HostBlock descriptors (extents only are needed after upload)
+        self.blockLevels = []
         self._keep = []
+        # nCellGlobal(level): the owned cells of a level over all ranks.  Formed from this rank's blocks on one rank; a
+        # multi-rank host sets it for each level it monitors.
+        self.nCellGlobal = {}
+        self.totalR0 = None   # getFreeStreamResidual's value, once per flow (freeStreamResSet)
+        self._totalR = 0.0    # the totalR last passed to setTotalResiduals
 
     # -- data model ---------------------------------------------------------
     def addBlock(self, hb, level=1, upload_metrics=True):
@@ -41,6 +105,7 @@ class ADFLOW_B200:
         if hb.subfaces:
             self.setBCData(blk, hb.subfaces)
         self.blocks.append(hb)
+        self.blockLevels.append(level)
         self.uploadState(blk, hb)
         return blk
 
@@ -397,13 +462,124 @@ class ADFLOW_B200:
 
     def resetFlow(self, mg_start_level, mu_inf, eddy_vis_inf_ratio):
         """_resetFlow (pyADflow.py:3097-3111): the ground level becomes mgStartLevel and its blocks get the uniform flow;
-        fullMultigridStartUp(mg_start_level, ...) then starts from there."""
+        fullMultigridStartUp(mg_start_level, ...) or solve(mg_start_level, ...) then starts from there.  The cached
+        free-stream residual totalR0 is forgotten (freeStreamResSet = .false.)."""
         self.setGroundLevel(mg_start_level)
         self.setUniformFlow(mg_start_level, mu_inf, eddy_vis_inf_ratio)
+        self.totalR0 = None
 
     def setTotalResiduals(self, totalR, totalR0):
         """iteration%totalR and totalR0, read by the dissipation-based continuation (useDissContinuation)."""
         check(self.L.adfb_set_total_residuals(float(totalR), float(totalR0)), "adfb_set_total_residuals")
+
+    # -- convergence monitor and the steady solver loop (src/solver/solvers.F90) -----------------------------------
+    def monitorSums(self, level=1, what=MON_SUMS | MON_MAXIMA):
+        """adfb_monitor: the ten all-reduced sums and maxima of the blocks of `level` (include/adflow_b200.h)"""
+        out = (C.c_double * 10)()
+        check(self.L.adfb_monitor(level, what, out), "adfb_monitor")
+        return np.array(list(out))
+
+    def _n_cell_global(self, level):
+        if level not in self.nCellGlobal:
+            if self.nranks > 1:
+                raise ValueError("nCellGlobal[%d] must be set on a multi-rank context" % level)
+            self.nCellGlobal[level] = sum(hb.d.nx * hb.d.ny * hb.d.nz for hb, lv in zip(self.blocks, self.blockLevels) if lv == level)
+        return self.nCellGlobal[level]
+
+    def _monitor(self, level, names):
+        what = MON_SUMS | (MON_MAXIMA if any(MONITOR_SLOTS[n] > 6 for n in names) else 0)
+        raw = self.monitorSums(level, what)
+        n = float(self._n_cell_global(level))
+        out = {}
+        for name in names:
+            q = MONITOR_SLOTS[name]
+            out[name] = math.sqrt(raw[q] / n) if q < 6 else math.sqrt(raw[q]) if q == 6 else float(raw[q])
+        return out
+
+    def monitor(self, level=1, names=DEFAULT_MONITOR_VARIABLES):
+        """The values convergenceInfo monitors on ground level `level` for the monitorVariables keywords `names`, as it
+        finishes them (solvers.F90:1642-1706), by CGNS name: a residual norm is sqrt(sum / nCellGlobal(level)), totalR is
+        sqrt(sum), the maxima as they are.  resrho and totalR are always there; "cpu" adds nothing here (solveState
+        records the host wall time)."""
+        return self._monitor(level, monitor_names(names, self.prm.equations == 3)[0])
+
+    def solveState(self, nCycles=2000, nCyclesCoarse=500, L2Convergence=1e-8, L2ConvergenceCoarse=1e-2, L2ConvergenceRel=1e-16,
+                   maxL2DeviationFactor=1.0, MGCycle="sg", smoother="DADI", nSubiter=1, monitorVariables=DEFAULT_MONITOR_VARIABLES):
+        """The steady solveState with the smoother on every iteration (solvers.F90:892-1236, neither ANK nor NK) on the
+        current ground level; the keyword arguments are the pyADflow options of the same names, with their defaults
+        (monitorVariables without cl and cd).  Returns {"converged", "failed", "history"}, the history as
+        getConvergenceHistory gives it (pyADflow.py:1404): "total minor iters", "iter type", "CFL", "step",
+        "linear res", "wall time" with "cpu", and one list per monitored CGNS name, iteration 0 first."""
+        if smoother not in ("DADI", "Runge-Kutta", "RK"):
+            raise ValueError("smoother must be 'DADI' or 'Runge-Kutta', got %r" % (smoother,))
+        sm = "DADI" if smoother == "DADI" else "RK"
+        names, cpu = monitor_names(monitorVariables, self.prm.equations == 3)
+        t0 = time.perf_counter()
+        ground = int(self.L.adfb_get_ground_level())
+        n_mg = nCycles if ground == 1 else nCyclesCoarse
+        cyc = self.cycleStrategy(MGCycle if ground == 1 else dict(self.fmgSchedule(ground, MGCycle))[ground])
+        if ground == 1 and self.totalR0 is None:
+            self.totalR0 = self.getFreeStreamResidual()
+        total_r0 = self.totalR0 if self.totalR0 is not None else 0.0
+        diss = bool(self.prm.useDissContinuation)
+        hist = {"total minor iters": [], "iter type": [], "CFL": [], "step": [], "linear res": []}
+        if cpu:
+            hist["wall time"] = []
+        for name in names:
+            hist[name] = []
+
+        def record(its, kind, cfl, step, vals):
+            # convergenceInfo stores the CFL and the step only when they are not negative (solvers.F90:1588-1620)
+            hist["total minor iters"].append(its)
+            hist["iter type"].append(kind)
+            hist["CFL"].append(max(cfl, 0.0))
+            hist["step"].append(max(step, 0.0))
+            hist["linear res"].append(0.0)
+            if cpu:
+                hist["wall time"].append(time.perf_counter() - t0)
+            for name in names:
+                hist[name].append(vals[name])
+            if diss:
+                self._totalR = vals["totalR"]
+                self.setTotalResiduals(self._totalR, total_r0)
+
+        def status(its, vals):
+            return convergence_status(ground, its, nCycles, [vals[n] for n in names], vals["RSDMassRMS"], rho_start, vals["totalR"],
+                                      total_r0, total_r_start, L2Convergence, L2ConvergenceCoarse, L2ConvergenceRel,
+                                      maxL2DeviationFactor)
+
+        if diss:   # the first residual reads the new totalR0 and the totalR of the last monitor
+            self.setTotalResiduals(self._totalR, total_r0)
+        # the first residual (blocketteRes with the store-wall flag, blockette.F90:135), then timeStep(.false.)
+        self.residual(RES_FLOW | RES_TURB | RES_STORE_WALL, level=ground)
+        self.timeStep(False, level=ground)
+        vals = self._monitor(ground, names)
+        rho_start, total_r_start = vals["RSDMassRMS"], vals["totalR"]
+        record(0, "None", -1.0, -1.0, vals)
+        converged, failed = False, any(math.isnan(vals[n]) for n in names)
+        its = 0
+        cfl = self.prm.cfl if ground == 1 else self.prm.cflCoarse
+        while its < n_mg and not failed:
+            self.mgCycle(cyc, sm, nSubiter)
+            its += 1
+            vals = self._monitor(ground, names)
+            record(its, sm, cfl, 1.0, vals)
+            converged, failed = status(its, vals)
+            if converged:
+                break
+        return {"converged": converged, "failed": failed, "history": hist}
+
+    def solve(self, mg_start_level, **options):
+        """The steady `solver` loop (solvers.F90:63-117): solveState(**options) on every ground level mgStartLevel .. 1,
+        transferToFineGrid(.false.) between them.  Returns [(groundLevel, result of solveState), ...]."""
+        out = []
+        for ground in range(mg_start_level, 0, -1):
+            self.setGroundLevel(ground)
+            out.append((ground, self.solveState(**options)))
+            if ground > 1:
+                self.mgProlongSolution(ground - 1)
+        self.setGroundLevel(1)
+        return out
 
     def getForces(self, ref_point=(0.0, 0.0, 0.0), p_ref=1.0, level=1):
         """Fp, Fv, Mp, Mv (rows) summed over the wall subfaces of all ranks -- wallIntegrationFace,

@@ -226,6 +226,23 @@ int adfb_residual(int level, unsigned flags);
 /* Sum of (dw(irho)/vol)^2 and of all (dw/vol)^2 over owned cells of all local
    blocks, all-reduced (getCurrentResidual, NKSolvers.F90:335-370). out[0]=rho, out[1]=total */
 int adfb_norms(double out[2]);
+/* The convergence monitor of convergenceInfo (solvers.F90:1338-1376, 1537-1545) on the live blocks of `level` of this
+   rank, all-reduced over the ranks (the sums with ncclSum, the maxima with ncclMax), over the owned cells 2:il, 2:jl, 2:kl:
+     out[0..5] sumResiduals (utils.F90:6364-6398): sum (dw(l) / vol)^2 for l = rho, rho u, rho v, rho w, rho E, nu~
+               (nu~ is 0 when nw == 5); a division, no iblank factor
+     out[6]    sumAllResiduals (:6400-6448): per cell, sum over l of (dw(l) ovv)^2 with ovv = 1 / vol and turbResScale on the
+               turbulence row, then added to the total
+     out[7]    hdiffMax of maxHdiffMach (:2466-2531): max |(rhoE + p) / rho - hInf| / hInf, hInf = (wInf(irhoE) + pInfCorr) / rhoInf
+     out[8]    MachMax: sqrt(max ((u^2 + v^2 + w^2) rho / (gamma p)))
+     out[9]    eddyvisMax of maxEddyv (:2422-2464): max(0, rev / rlv), 0 unless the equations are RANS
+   what: bit 0 the sums (out[0..6]), bit 1 the maxima (out[7..9]); the entries of a cleared bit are 0 and their loads are
+   skipped.  The device's level-l blocks hold their own dw: on a coarse ground level it is that level's residual (see
+   DESIGN.md section 6).  Reproducible: a fixed partition per block, a fixed tree, the blocks combined in block-id order,
+   so one input gives the same bits on every call; the maxima are the reference's bits (cell values formed with
+   explicit roundings).  A NaN in dw makes the sums NaN; the maxima ignore NaN cells (fmax), so they may stay finite.
+   One host synchronisation per call.  Fails on a null out, a `what` other than 1, 2, 3, no adfb_set_params, or no live
+   block of `level`.  adfb_norms is out[0] and out[6] of level 1, bit for bit. */
+int adfb_monitor(int level, unsigned what, double out[10]);
 /* iteration%totalR and totalR0 (convergenceInfo, solvers.F90:1672; getFreeStreamResidual): the L2 norm of the current
    residual and of the free-stream residual, the same all-reduced values on every rank.  Only the dissipation-based
    continuation reads them; the host calls this after its convergence monitor and after adfb_free_stream_residual.
