@@ -50,6 +50,11 @@ struct Block {
     double* saved = nullptr;   // w, p, rlv, rev kept by adfb_free_stream_residual (in allocs)
 };
 
+// the matrix-free operators that share the device vectors nkA, nkU, nkF0, nkY (kMfOps)
+enum { MF_NONE = -1, MF_NK, MF_ANK, MF_ANK_TURB };
+// reduction scratch: 2 x 1024 partials and two results; host-read values, at most 256 at a time
+const int kDRedN = 2 * 1024 + 2, kHRedN = 256;
+
 struct Context {
     bool ready = false;
     int device = -1, rank = 0, nranks = 1;
@@ -65,18 +70,18 @@ struct Context {
     AdfbParams prm;
     bool havePrm = false;
     std::vector<Block> blocks;
-    double* dRed = nullptr;   // reduction scratch
-    size_t dRedN = 0;
+    double* dRed = nullptr;   // reduction scratch (kDRedN)
     double* dMon = nullptr;   // monitor partials, one slot per block of the level, and the results
     size_t dMonN = 0;
-    double* hRed = nullptr;   // pinned
+    double* hRed = nullptr;   // pinned (kHRedN)
     double* dVec = nullptr;   // AoS staging vector (get/set states, get res)
     size_t dVecN = 0;
-    // NK / MFFD device vectors: direction a, base state U, base residual F(U), result y
+    // device vectors of the matrix-free products (NK, ANK, ANK turbulence): direction a, base state U, base residual
+    // F(U), result y; the operator whose base U, F0 hold, ||U|| and the h of the last NK or ANK product
     double *nkA = nullptr, *nkU = nullptr, *nkF0 = nullptr, *nkY = nullptr;
     size_t nkN = 0;
-    bool nkHaveBase = false;
-    double nkUnorm = 0.0, nkLastH = 0.0;
+    int mfOwner = MF_NONE;
+    double mfUnorm = 0.0, nkLastH = 0.0;
     MffdDev* dMffd = nullptr;     // record of the fused matrix-free product (device) and its pinned host image
     MffdDev* hMffd = nullptr;
     bool mffdFuse = false;        // adfb_residual: skip k_state_prep (done by k_nkvec_prep) and form y in the kernels that write dw
@@ -114,10 +119,9 @@ struct Context {
     bool capturing = false;
     // ANK (module ANKSolver): options, per-cell time-step blocks, the perturbed vector of the last product
     AdfbAnkParams ank;
-    bool haveAnk = false, ankHaveT = false, ankHaveBase = false, ankTurbHaveBase = false;
+    bool haveAnk = false, ankHaveT = false;
     double *ankT = nullptr, *ankPert = nullptr;
     size_t ankTN = 0, ankPertN = 0;
-    double ankUnorm = 0.0;
     // device GMRES workspace: (restart + 2) vectors + reduction scratch
     double *kryV = nullptr, *kryRed = nullptr;
     size_t kryVN = 0;
@@ -324,7 +328,8 @@ int create_device_resources() {
     for (cudaEvent_t* e : {&g.evPost, &g.evDone}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     for (auto& row : g.ffEv) for (cudaEvent_t& e : row) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     CK(cudaMalloc((void**)&g.dConst, 8 * sizeof(double)));
-    CK(cudaMallocHost((void**)&g.hRed, 256 * sizeof(double)));
+    CK(cudaMalloc((void**)&g.dRed, kDRedN * sizeof(double)));
+    CK(cudaMallocHost((void**)&g.hRed, kHRedN * sizeof(double)));
     return 0;
 }
 void release_device_resources() {
@@ -333,8 +338,31 @@ void release_device_resources() {
     for (cudaStream_t* s : {&g.stream, &g.commStream, &g.ffIn, &g.ffOut, &g.ffBack}) { if (*s) cudaStreamDestroy(*s); *s = nullptr; }
     if (g.dConst) cudaFree(g.dConst);
     g.dConst = nullptr;
+    if (g.dRed) cudaFree(g.dRed);
+    g.dRed = nullptr;
     if (g.hRed) cudaFreeHost(g.hRed);
     g.hRed = nullptr;
+}
+
+// The host-read tail of a reduction: the n values at dev, all-reduced over the ranks with the NCCL operation op, reach
+// the host through the pinned buffer after one synchronisation of the library stream.
+int allreduce(double* dev, int n, int op) {
+    if (g.nranks > 1) {
+        const int rc = g.nccl.AllReduce(dev, dev, n, kNcclDouble, op, g.comm, g.stream);
+        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
+    }
+    return 0;
+}
+int fetch(const double* dev, int n, double* out) {
+    if (n < 0 || n > kHRedN) return fail("reduction of %d values does not fit the %d-value host buffer", n, kHRedN);
+    CK(cudaMemcpyAsync(g.hRed, dev, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
+    CK(cudaStreamSynchronize(g.stream));
+    for (int i = 0; i < n; i++) out[i] = g.hRed[i];
+    return 0;
+}
+int allreduce_fetch(double* dev, int n, int op, double* out) {
+    if (allreduce(dev, n, op)) return 1;
+    return fetch(dev, n, out);
 }
 
 }  // namespace
@@ -429,8 +457,6 @@ int adfb_finalize(void) {
     for (size_t i = 0; i < g.blocks.size(); i++)
         if (g.blocks[i].alive) adfb_block_destroy((int)i);
     g.blocks.clear();
-    if (g.dRed) cudaFree(g.dRed);
-    g.dRed = nullptr; g.dRedN = 0;
     if (g.dMon) cudaFree(g.dMon);
     g.dMon = nullptr; g.dMonN = 0;
     if (g.dMffd) { cudaFree(g.dMffd); g.dMffd = nullptr; }
@@ -439,11 +465,11 @@ int adfb_finalize(void) {
     g.dVec = nullptr; g.dVecN = 0;
     for (double** p : {&g.nkA, &g.nkU, &g.nkF0, &g.nkY}) { if (*p) cudaFree(*p); *p = nullptr; }
     g.nkN = 0;
-    g.nkHaveBase = false; g.ankHaveBase = false; g.ankTurbHaveBase = false;   // the base vectors went with the buffers g.nkHaveBase = false;
+    g.mfOwner = MF_NONE;   // the base vectors went with the buffers
     // ANK / Krylov state belongs to the context as well: a later adfb_init starts from scratch
     for (double** p : {&g.ankT, &g.ankPert, &g.kryV, &g.kryRed}) { if (*p) cudaFree(*p); *p = nullptr; }
     g.ankTN = 0; g.ankPertN = 0; g.kryVN = 0;
-    g.haveAnk = false; g.ankHaveT = false; g.ankHaveBase = false;
+    g.haveAnk = false; g.ankHaveT = false;
     // so do the parameters and the multigrid position: a later context starts on ground level 1 and must set its parameters
     g.havePrm = false;
     g.groundLevel = 1; g.mgInitWr = 1;
@@ -1132,13 +1158,15 @@ static int nk_buffers(long long need) {
     if (g.nkN >= (size_t)need) return 0;
     for (double** p : {&g.nkA, &g.nkU, &g.nkF0, &g.nkY}) { if (*p) cudaFree(*p); *p = nullptr; }
     g.nkN = 0;
-    g.nkHaveBase = false; g.ankHaveBase = false; g.ankTurbHaveBase = false;   // the base vectors went with the buffers
+    g.mfOwner = MF_NONE;   // the base vectors went with the buffers
     for (double** p : {&g.nkA, &g.nkU, &g.nkF0, &g.nkY}) CK(cudaMalloc((void**)p, need * sizeof(double)));
-    if (!g.dRed) { CK(cudaMalloc((void**)&g.dRed, (2 * 1024 + 2) * sizeof(double))); g.dRedN = 2 * 1024 + 2; }
     g.nkN = need;
     return 0;
 }
-static int nk_vec_kernel(const double* vec, const double* base, double* out, double h, int mode) {
+// The vector pass of a matrix-free operator (kMfOps) over the owned cells of level 1, with vec the state set in modes 0
+// and 2 and the direction in mode 1: mode 0 sets w, 1 perturbs w = U + h a, 2 writes R into out, 3 writes (R - F0) / h.
+static int nk_vec_kernel(int mode, const double* vec, const double* base, double* out, double h) {
+    if (mode >= 2) vec = nullptr;   // k_nkvec reads only the residual in modes 2 and 3
     long long off = 0;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
@@ -1161,14 +1189,7 @@ static int nk_sumsq(const double* v, long long n, double* out) {
     KT_BEGIN(K_MFFD, g.stream);
     k_sum_final<<<1, 256, 0, g.stream>>>(g.dRed, nPart);
     KT_END(K_MFFD, g.stream);
-    if (g.nranks > 1) {
-        const int rc = g.nccl.AllReduce(g.dRed + nPart, g.dRed + nPart, 1, kNcclDouble, kNcclSum, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, g.dRed + nPart, sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    *out = g.hRed[0];
-    return 0;
+    return allreduce_fetch(g.dRed + nPart, 1, kNcclSum, out);
 }
 static const unsigned kNkFlags = ADFB_RES_FLOW | ADFB_RES_TURB;
 
@@ -1341,146 +1362,52 @@ static int form_function_pipelined(const double* wVec, double* rVec, long long n
     return 0;
 }
 
-// FormFunction_mf (NKSolvers.F90:437-461): setW(wVec); computeResidualNK; setRVec(rVec)
-int adfb_form_function(const double* wVec, double* rVec, long long n) {
-    ADFB_RANGE("adfb_form_function");
-    NEED_INIT();
-    if (!g.havePrm) return fail("adfb_form_function: adfb_set_params has not been called");
+// parameters set, vectors of the local state size, buffers that hold them
+static int nk_check(const char* who, bool vecs, long long n) {
+    if (!g.havePrm) return fail("%s: adfb_set_params has not been called", who);
     const long long need = adfb_state_size();
-    if (!wVec || !rVec || n != need) return fail("adfb_form_function: vector length %lld != local state size %lld", n, need);
-    if (nk_buffers(need)) return 1;
-    for (Block& b : g.blocks)
-        if (b.alive && b.level == 1 && !b.haveMetrics) return fail("adfb_form_function: geometry of a block was never set");
-    {
-        const int rc = form_function_pipelined(wVec, rVec, need);
-        if (rc >= 0) return rc;
-    }
-    CK(cudaMemcpyAsync(g.nkA, wVec, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (nk_vec_kernel(g.nkA, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, kNkFlags)) return 1;
-    if (nk_vec_kernel(nullptr, nullptr, g.nkY, 1.0, 2)) return 1;
-    CK(cudaMemcpyAsync(rVec, g.nkY, need * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
+    if (!vecs || n != need) return fail("%s: vector length %lld != local state size %lld", who, n, need);
+    return nk_buffers(need);
 }
 
-// MatMFFDSetBase(dRdw, wVec, baseRes) (NKSolvers.F90:628-630): U <- wVec, F0 <- F(U) on the device
-int adfb_mffd_set_base(const double* U, long long n) {
-    ADFB_RANGE("adfb_mffd_set_base");
-    NEED_INIT();
-    if (!g.havePrm) return fail("adfb_mffd_set_base: adfb_set_params has not been called");
-    const long long need = adfb_state_size();
-    if (!U || n != need) return fail("adfb_mffd_set_base: vector length %lld != local state size %lld", n, need);
-    if (nk_buffers(need)) return 1;
-    CK(cudaMemcpyAsync(g.nkU, U, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (nk_vec_kernel(g.nkU, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, kNkFlags)) return 1;
-    if (nk_vec_kernel(nullptr, nullptr, g.nkF0, 1.0, 2)) return 1;
-    double uu = 0.0;
-    if (nk_sumsq(g.nkU, need, &uu)) return 1;
-    g.nkUnorm = sqrt(uu);
-    g.nkHaveBase = true;
-    g.ankHaveBase = false; g.ankTurbHaveBase = false;   // the ANK bases share the buffers
-    return 0;
-}
-
-// MatMult of the MFFD shell: y = (F(U + h a) - F(U)) / h.  h > 0: use it as given;
-// h <= 0: PETSc's default Walker-Pernice choice h = error_rel * sqrt(1 + ||U||) / ||a||
-// with error_rel = sqrt(machine epsilon) (PARITY UNPINNED at this boundary, see DESIGN.md).
-// y = (F(U + h a) - F(U)) / h with a in g.nkA, y into g.nkY (device); returns 2 when a == 0 (y = 0, no residual)
-static int mffd_core(long long need, double h) {
-    if (h <= 0.0) {
-        double aa = 0.0;
-        if (nk_sumsq(g.nkA, need, &aa)) return 1;
-        if (aa == 0.0) {
-            g.nkLastH = 0.0;
-            return 2;
-        }
-        h = 1.4901161193847656e-08 * sqrt(1.0 + g.nkUnorm) / sqrt(aa);
-    }
-    g.nkLastH = h;
-    // fused form (NKSolvers.F90:437-461 in one pass each way): the perturbation is formed together with p / rlv / rev of
-    // the owned cells, and the kernels that write dw (tile kernel, k_sa) form y = (R - F0) / h of their rows; bitwise
-    // the unfused product (same operations on the same operands).  ADFB_MFFD_FUSED=0, or a block the tile kernel does not
-    // take (matrix / upwind dissipation, coarse level), selects the three-pass form.
-    // The two extra vector passes of the three-pass form cost less than the strided AoS accesses of the epilogue inside
-    // the tile kernel (the product is not bandwidth bound), so the three-pass form stays the default; ADFB_MFFD_FUSED=1
-    // selects the fused one.
+// The NK product y = (F(U + h a) - F(U)) / h in its fused form (NKSolvers.F90:437-461 in one pass each way): the
+// perturbation is formed together with p / rlv / rev of the owned cells, and the kernels that write dw (tile kernel, k_sa)
+// form y = (R - F0) / h of their rows; bitwise the unfused product (same operations on the same operands).
+// ADFB_MFFD_FUSED=0, or a block the tile kernel does not take (matrix / upwind dissipation, coarse level), selects the
+// three-pass form: returns -1.
+// The two extra vector passes of the three-pass form cost less than the strided AoS accesses of the epilogue inside
+// the tile kernel (the product is not bandwidth bound), so the three-pass form stays the default; ADFB_MFFD_FUSED=1
+// selects the fused one.
+static int nk_mffd_fused(double h) {
     bool fuse = false;
     { const char* e = getenv("ADFB_MFFD_FUSED"); if (e && e[0] == '1') fuse = true; }
     if (g_kt.on) fuse = false;
     for (Block& b : g.blocks)
         if (b.alive && b.level == 1 && !tile_kernel_applies(b.d, b.dev, residual_discr(1, true))) fuse = false;
     if (overset_present(1)) fuse = false;   // the exchange rewrites owned fringe cells: p, rhoE must follow (k_etot_owned)
-    if (fuse) {
-        if (!g.dMffd) {
-            CK(cudaMalloc((void**)&g.dMffd, sizeof(MffdDev)));
-            CK(cudaMallocHost((void**)&g.hMffd, sizeof(MffdDev)));
-        }
-        int nw0 = 6;
-        for (Block& b : g.blocks) if (b.alive && b.level == 1) { nw0 = b.nw; break; }
-        g.hMffd->F0 = g.nkF0; g.hMffd->y = g.nkY; g.hMffd->h = h; g.hMffd->nw = nw0;
-        CK(cudaMemcpyAsync(g.dMffd, g.hMffd, sizeof(MffdDev), cudaMemcpyHostToDevice, g.stream));
-        long long off = 0;
-        for (Block& b : g.blocks) {
-            if (!b.alive || b.level != 1) continue;
-            const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz;
-            KT_BEGIN(K_MFFD, g.stream);
-            k_nkvec_prep<<<(unsigned)((nc + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, b.nw, g.nkA + off, g.nkU + off, g.dMffd, 1);
-            KT_END(K_MFFD, g.stream);
-            off += nc * b.nw;
-        }
-        g.mffdFuse = true;
-        const int rc = adfb_residual(1, kNkFlags);
-        g.mffdFuse = false;
-        return rc ? 1 : 0;
+    if (!fuse) return -1;
+    if (!g.dMffd) {
+        CK(cudaMalloc((void**)&g.dMffd, sizeof(MffdDev)));
+        CK(cudaMallocHost((void**)&g.hMffd, sizeof(MffdDev)));
     }
-    if (nk_vec_kernel(g.nkA, g.nkU, nullptr, h, 1)) return 1;
-    if (adfb_residual(1, kNkFlags)) return 1;
-    if (nk_vec_kernel(nullptr, g.nkF0, g.nkY, h, 3)) return 1;
-    return 0;
-}
-int adfb_mffd_apply(const double* a, double* y, long long n, double h) {
-    ADFB_RANGE("adfb_mffd_apply");
-    NEED_INIT();
-    if (!g.nkHaveBase) return fail("adfb_mffd_apply: adfb_mffd_set_base has not been called");
-    const long long need = adfb_state_size();
-    if (!a || !y || n != need || (size_t)need > g.nkN) return fail("adfb_mffd_apply: vector length %lld != local state size %lld", n, need);
-    CK(cudaMemcpyAsync(g.nkA, a, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    const int rc = mffd_core(need, h);
-    if (rc == 1) return 1;
-    if (rc == 2) {
-        CK(cudaStreamSynchronize(g.stream));
-        memset(y, 0, need * sizeof(double));
-        return 0;
+    int nw0 = 6;
+    for (Block& b : g.blocks) if (b.alive && b.level == 1) { nw0 = b.nw; break; }
+    g.hMffd->F0 = g.nkF0; g.hMffd->y = g.nkY; g.hMffd->h = h; g.hMffd->nw = nw0;
+    CK(cudaMemcpyAsync(g.dMffd, g.hMffd, sizeof(MffdDev), cudaMemcpyHostToDevice, g.stream));
+    long long off = 0;
+    for (Block& b : g.blocks) {
+        if (!b.alive || b.level != 1) continue;
+        const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz;
+        KT_BEGIN(K_MFFD, g.stream);
+        k_nkvec_prep<<<(unsigned)((nc + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, b.nw, g.nkA + off, g.nkU + off, g.dMffd, 1);
+        KT_END(K_MFFD, g.stream);
+        off += nc * b.nw;
     }
-    CK(cudaMemcpyAsync(y, g.nkY, need * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
+    g.mffdFuse = true;
+    const int rc = adfb_residual(1, kNkFlags);
+    g.mffdFuse = false;
+    return rc ? 1 : 0;
 }
-// the same product for Krylov vectors that already live on THIS device (PETSc VECCUDA: VecCUDAGetArrayRead /
-// VecCUDAGetArrayWrite): no PCIe traffic; the result is complete when the call returns
-int adfb_mffd_apply_device(const double* aDev, double* yDev, long long n, double h) {
-    ADFB_RANGE("adfb_mffd_apply_device");
-    NEED_INIT();
-    if (!g.nkHaveBase) return fail("adfb_mffd_apply_device: adfb_mffd_set_base has not been called");
-    const long long need = adfb_state_size();
-    if (!aDev || !yDev || n != need || (size_t)need > g.nkN)
-        return fail("adfb_mffd_apply_device: vector length %lld != local state size %lld", n, need);
-    cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, aDev) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
-        return fail("adfb_mffd_apply_device: a is not a device pointer of device %d", g.device);
-    if (cudaPointerGetAttributes(&at, yDev) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
-        return fail("adfb_mffd_apply_device: y is not a device pointer of device %d", g.device);
-    CK(cudaMemcpyAsync(g.nkA, aDev, need * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-    const int rc = mffd_core(need, h);
-    if (rc == 1) return 1;
-    if (rc == 2) CK(cudaMemsetAsync(yDev, 0, need * sizeof(double), g.stream));
-    else CK(cudaMemcpyAsync(yDev, g.nkY, need * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
-}
-double adfb_mffd_last_h(void) { return g.nkLastH; }
 
 // referenceShockSensor, src/adjoint/adjointUtils.F90:1900-1950
 int adfb_reference_shock_sensor(int level) {
@@ -1704,7 +1631,8 @@ int adfb_ank_set_params(const AdfbAnkParams* ank) {
     // No drop_graphs: the ANK products launch their own kernels with g.ank as an argument at every call, and the residual
     // they call is keyed by its flags, which carry the ANK options it depends on (ank_res_flags).
     g.ank = *ank;
-    g.haveAnk = true; g.ankHaveT = false; g.ankHaveBase = false;
+    g.haveAnk = true; g.ankHaveT = false;
+    if (g.mfOwner == MF_ANK) g.mfOwner = MF_NONE;
     return 0;
 }
 int adfb_ank_time_step_mat(void) {
@@ -1735,7 +1663,10 @@ int adfb_ank_time_step_mat(void) {
     g.ankHaveT = true;
     return 0;
 }
-static int ank_vec_kernel(const double* vec, const double* base, double* out, double* pert, double h, int mode) {
+// the vector pass of the ANK operator (modes of nk_vec_kernel; mode 4: out = T vec with the time-step matrix T)
+static int ank_vec_kernel(int mode, const double* vec, const double* base, double* out, double h) {
+    double* pert = mode == 1 ? g.ankPert : nullptr;   // the perturbed state of mode 1 is what mode 3 differences against
+    if (mode == 3) vec = g.ankPert;
     long long off = 0;
     size_t offT = 0;
     for (Block& b : g.blocks) {
@@ -1753,102 +1684,25 @@ static int ank_vec_kernel(const double* vec, const double* base, double* out, do
     CK(cudaGetLastError());
     return 0;
 }
-static int ank_ready(const char* who, long long n, long long* need) {
-    if (!g.havePrm || !g.haveAnk) return fail("%s: adfb_set_params / adfb_ank_set_params have not been called", who);
-    if (!g.ankHaveT) return fail("%s: adfb_ank_time_step_mat has not been called", who);
-    *need = ank_vec_size();
-    if (n != *need) return fail("%s: vector length %lld != %lld (nState entries per owned cell)", who, n, *need);
+// the shared vectors and the perturbed state (n entries) of the ANK products
+static int ank_buffers(long long n) {
     if (nk_buffers(adfb_state_size())) return 1;
-    if (g.ankPertN < (size_t)*need) {
+    if (g.ankPertN < (size_t)n) {
         if (g.ankPert) cudaFree(g.ankPert);
         g.ankPert = nullptr; g.ankPertN = 0;
-        CK(cudaMalloc((void**)&g.ankPert, *need * sizeof(double)));
-        g.ankPertN = *need;
+        CK(cudaMalloc((void**)&g.ankPert, n * sizeof(double)));
+        g.ankPertN = n;
     }
     return 0;
 }
-// FormFunction_mf (:2468-2538)
-int adfb_ank_form_function(const double* inVec, double* rVec, long long n) {
-    ADFB_RANGE("adfb_ank_form_function");
-    NEED_INIT();
-    long long need = 0;
-    if (!inVec || !rVec) return fail("adfb_ank_form_function: null vector");
-    if (ank_ready("adfb_ank_form_function", n, &need)) return 1;
-    CK(cudaMemcpyAsync(g.nkA, inVec, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (ank_vec_kernel(g.nkA, nullptr, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, ank_res_flags())) return 1;
-    if (ank_vec_kernel(g.nkA, nullptr, g.nkY, nullptr, 1.0, 2)) return 1;
-    CK(cudaMemcpyAsync(rVec, g.nkY, need * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
+static int ank_check(const char* who, bool vecs, long long n) {
+    if (!vecs) return fail("%s: null vector", who);
+    if (!g.havePrm || !g.haveAnk) return fail("%s: adfb_set_params / adfb_ank_set_params have not been called", who);
+    if (!g.ankHaveT) return fail("%s: adfb_ank_time_step_mat has not been called", who);
+    const long long need = ank_vec_size();
+    if (n != need) return fail("%s: vector length %lld != %lld (nState entries per owned cell)", who, n, need);
+    return ank_buffers(need);
 }
-int adfb_ank_mffd_set_base(const double* U, long long n) {
-    NEED_INIT();
-    long long need = 0;
-    if (!U) return fail("adfb_ank_mffd_set_base: null vector");
-    if (ank_ready("adfb_ank_mffd_set_base", n, &need)) return 1;
-    CK(cudaMemcpyAsync(g.nkU, U, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (ank_vec_kernel(g.nkU, nullptr, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, ank_res_flags())) return 1;
-    if (ank_vec_kernel(g.nkU, nullptr, g.nkF0, nullptr, 1.0, 2)) return 1;
-    double uu = 0.0;
-    if (nk_sumsq(g.nkU, need, &uu)) return 1;
-    g.ankUnorm = sqrt(uu);
-    g.ankHaveBase = true;
-    g.nkHaveBase = false; g.ankTurbHaveBase = false;   // the NK base shares the buffers
-    return 0;
-}
-// y = (F(U + h a) - F(U)) / h with a in g.nkA, y into g.nkY; returns 2 when a == 0
-static int ank_mffd_core(long long need, double h) {
-    if (h <= 0.0) {
-        double aa = 0.0;
-        if (nk_sumsq(g.nkA, need, &aa)) return 1;
-        if (aa == 0.0) { g.nkLastH = 0.0; return 2; }
-        h = 1.4901161193847656e-08 * sqrt(1.0 + g.ankUnorm) / sqrt(aa);
-    }
-    g.nkLastH = h;
-    if (ank_vec_kernel(g.nkA, g.nkU, nullptr, g.ankPert, h, 1)) return 1;
-    if (adfb_residual(1, ank_res_flags())) return 1;
-    if (ank_vec_kernel(g.ankPert, g.nkF0, g.nkY, nullptr, h, 3)) return 1;
-    return 0;
-}
-int adfb_ank_mffd_apply(const double* a, double* y, long long n, double h) {
-    ADFB_RANGE("adfb_ank_mffd_apply");
-    NEED_INIT();
-    long long need = 0;
-    if (!a || !y) return fail("adfb_ank_mffd_apply: null vector");
-    if (ank_ready("adfb_ank_mffd_apply", n, &need)) return 1;
-    if (!g.ankHaveBase) return fail("adfb_ank_mffd_apply: adfb_ank_mffd_set_base has not been called");
-    CK(cudaMemcpyAsync(g.nkA, a, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    const int rc = ank_mffd_core(need, h);
-    if (rc == 1) return 1;
-    if (rc == 2) { CK(cudaStreamSynchronize(g.stream)); memset(y, 0, need * sizeof(double)); return 0; }
-    CK(cudaMemcpyAsync(y, g.nkY, need * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
-}
-// the same product for Krylov vectors resident on this device (PETSc VECCUDA), like adfb_mffd_apply_device
-int adfb_ank_mffd_apply_device(const double* aDev, double* yDev, long long n, double h) {
-    ADFB_RANGE("adfb_ank_mffd_apply_device");
-    NEED_INIT();
-    long long need = 0;
-    if (!aDev || !yDev) return fail("adfb_ank_mffd_apply_device: null vector");
-    if (ank_ready("adfb_ank_mffd_apply_device", n, &need)) return 1;
-    if (!g.ankHaveBase) return fail("adfb_ank_mffd_apply_device: adfb_ank_mffd_set_base has not been called");
-    cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, aDev) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
-        return fail("adfb_ank_mffd_apply_device: a is not a device pointer of device %d", g.device);
-    if (cudaPointerGetAttributes(&at, yDev) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
-        return fail("adfb_ank_mffd_apply_device: y is not a device pointer of device %d", g.device);
-    CK(cudaMemcpyAsync(g.nkA, aDev, need * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-    const int rc = ank_mffd_core(need, h);
-    if (rc == 1) return 1;
-    if (rc == 2) CK(cudaMemsetAsync(yDev, 0, need * sizeof(double), g.stream));
-    else CK(cudaMemcpyAsync(yDev, g.nkY, need * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
-}
-// physicalityCheckANK (:3013-3210)
 // ---- turbulence KSP of the decoupled ANK (ANKTurbSolveKSP, NKSolvers.F90:3337 ff.): one turbulence variable per owned cell
 static long long ank_turb_vec_size(void) {
     long long n = 0;
@@ -1856,19 +1710,13 @@ static long long ank_turb_vec_size(void) {
         if (b.alive && b.level == 1) n += (long long)b.d.nx * b.d.ny * b.d.nz;
     return n;
 }
-static int ank_turb_ready(const char* who, long long n) {
+static int ank_turb_check(const char* who, bool vecs, long long n) {
+    if (!vecs) return fail("%s: null vector", who);
     if (!g.havePrm || !g.haveAnk) return fail("%s: adfb_set_params / adfb_ank_set_params have not been called", who);
     if (g.prm.equations != ADFB_RANS) return fail("%s: needs the RANS equations (a turbulence variable)", who);
     const long long need = ank_turb_vec_size();
     if (n != need) return fail("%s: vector length %lld != %lld (one turbulence variable per owned cell)", who, n, need);
-    if (nk_buffers(adfb_state_size())) return 1;
-    if (g.ankPertN < (size_t)need) {
-        if (g.ankPert) cudaFree(g.ankPert);
-        g.ankPert = nullptr; g.ankPertN = 0;
-        CK(cudaMalloc((void**)&g.ankPert, need * sizeof(double)));
-        g.ankPertN = need;
-    }
-    return 0;
+    return ank_buffers(need);
 }
 // blocketteRes without useUpdateIntermed leaves the block's dtl alone (the tile's time step stays local, blockette.F90:1929),
 // the device residual always stores it: the time-stepping term uses the copy taken before the residual (work array 0)
@@ -1879,7 +1727,10 @@ static int ank_turb_save_dtl(void) {
     }
     return 0;
 }
-static int ank_turb_vec_kernel(const double* vec, const double* base, double* out, double* pert, double h, int mode) {
+// the vector pass of the ANK turbulence operator (modes of nk_vec_kernel)
+static int ank_turb_vec_kernel(int mode, const double* vec, const double* base, double* out, double h) {
+    double* pert = mode == 1 ? g.ankPert : nullptr;
+    if (mode == 3) vec = g.ankPert;
     long long off = 0;
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
@@ -1893,78 +1744,218 @@ static int ank_turb_vec_kernel(const double* vec, const double* base, double* ou
     CK(cudaGetLastError());
     return 0;
 }
-// FormFunction_mf_turb (:2540-2612): setWANK(inVec, nt1, nt2); blocketteRes(useFlowRes = .false.); setRVecANKTurb; time-stepping term
-int adfb_ank_form_function_turb(const double* inVec, double* rVec, long long n) {
-    ADFB_RANGE("adfb_ank_form_function_turb");
-    NEED_INIT();
-    if (!inVec || !rVec) return fail("adfb_ank_form_function_turb: null vector");
-    if (ank_turb_ready("adfb_ank_form_function_turb", n)) return 1;
-    CK(cudaMemcpyAsync(g.nkA, inVec, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (ank_turb_save_dtl()) return 1;
-    if (ank_turb_vec_kernel(g.nkA, nullptr, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, ADFB_RES_TURB)) return 1;
-    if (ank_turb_vec_kernel(g.nkA, nullptr, g.nkY, nullptr, 1.0, 2)) return 1;
-    CK(cudaMemcpyAsync(rVec, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
+
+// ---------------------------------------------------------------------------
+// The matrix-free operators on the shared vectors nkA, nkU, nkF0, nkY: the NK residual (FormFunction_mf,
+// NKSolvers.F90:437-461), the ANK flow or coupled residual (:2468-2538) and the ANK turbulence residual
+// (FormFunction_mf_turb, :2540-2612: setWANK; blocketteRes(useFlowRes = .false.); setRVecANKTurb; time-stepping term), each
+// with its PETSc MatMFFD product y = (F(U + h a) - F(U)) / h about a base U (MatMFFDSetBase, :628-630).  What differs:
+struct MfOp {
+    const char* setBase;   // the entry point that forms the base, named when a product finds none of its own
+    long long (*size)();   // local vector length
+    // parameters, vector length and buffers (vecs: no vector is null).  Products run it before they test the base when
+    // checkFirst: it may grow the buffers, which drops the base.  NK tests its base first, then the vectors against the
+    // buffers the base was formed in.
+    int (*check)(const char* who, bool vecs, long long n);
+    bool checkFirst;
+    unsigned (*flags)();   // of the residual
+    int (*vec)(int mode, const double* vec, const double* base, double* out, double h);   // modes of nk_vec_kernel
+    // h <= 0 takes PETSc's Walker-Pernice h from ||U||, which set_base forms, and adfb_mffd_last_h reports the h of the
+    // product; otherwise h <= 0 is refused
+    bool chooseH;
+    int (*preResidual)();    // before the residual of a function evaluation, or nullptr
+    int (*fused)(double h);  // the product in a single pass, -1 where it does not apply; or nullptr
+};
+static const MfOp kMfOps[] = {
+    {"adfb_mffd_set_base", adfb_state_size, nk_check, false, [] { return kNkFlags; }, nk_vec_kernel, true, nullptr, nk_mffd_fused},
+    {"adfb_ank_mffd_set_base", ank_vec_size, ank_check, true, ank_res_flags, ank_vec_kernel, true, nullptr, nullptr},
+    {"adfb_ank_mffd_turb_set_base", ank_turb_vec_size, ank_turb_check, true, [] { return (unsigned)ADFB_RES_TURB; }, ank_turb_vec_kernel,
+     false, ank_turb_save_dtl, nullptr},
+};
+
+// w <- x through xDev, yDev <- R(w): the function evaluation of the form function and of set_base
+static int mf_eval(const MfOp& op, const double* x, double* xDev, double* yDev, long long n) {
+    CK(cudaMemcpyAsync(xDev, x, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
+    if (op.preResidual && op.preResidual()) return 1;
+    if (op.vec(0, xDev, nullptr, nullptr, 0.0)) return 1;
+    if (adfb_residual(1, op.flags())) return 1;
+    return op.vec(2, xDev, nullptr, yDev, 1.0);
+}
+static int mf_form_function(int k, const double* x, double* r, long long n) {
+    if (mf_eval(kMfOps[k], x, g.nkA, g.nkY, n)) return 1;
+    CK(cudaMemcpyAsync(r, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
-// the matrix-free product of the turbulence KSP (MatMFFD shell over FormFunction_mf_turb): base state, then
-// y = (F(U + h a) - F(U)) / h with a given h > 0
+// U <- x, F0 <- F(U) on the device; the operator owns the vectors from here on
+static int mf_set_base(int k, const double* U, long long n) {
+    const MfOp& op = kMfOps[k];
+    g.mfOwner = MF_NONE;   // U and F0 are overwritten
+    if (mf_eval(op, U, g.nkU, g.nkF0, n)) return 1;
+    if (op.chooseH) {
+        double uu = 0.0;
+        if (nk_sumsq(g.nkU, n, &uu)) return 1;
+        g.mfUnorm = sqrt(uu);
+    } else {
+        CK(cudaStreamSynchronize(g.stream));
+    }
+    g.mfOwner = k;
+    return 0;
+}
+// MatMult of the MFFD shell: y = (F(U + h a) - F(U)) / h with a in g.nkA, y into g.nkY (device).  h > 0: use it as given;
+// h <= 0: PETSc's default Walker-Pernice choice h = error_rel * sqrt(1 + ||U||) / ||a|| with error_rel = sqrt(machine
+// epsilon) (PARITY UNPINNED at this boundary, see DESIGN.md).  Returns 2 when a == 0 (y = 0, no residual).
+static int mf_product(int k, long long n, double h) {
+    const MfOp& op = kMfOps[k];
+    if (op.chooseH) {
+        if (h <= 0.0) {
+            double aa = 0.0;
+            if (nk_sumsq(g.nkA, n, &aa)) return 1;
+            if (aa == 0.0) {
+                g.nkLastH = 0.0;
+                return 2;
+            }
+            h = 1.4901161193847656e-08 * sqrt(1.0 + g.mfUnorm) / sqrt(aa);
+        }
+        g.nkLastH = h;
+    }
+    if (op.fused) {
+        const int rc = op.fused(h);
+        if (rc >= 0) return rc;
+    }
+    if (op.vec(1, g.nkA, g.nkU, nullptr, h)) return 1;
+    if (adfb_residual(1, op.flags())) return 1;
+    return op.vec(3, nullptr, g.nkF0, g.nkY, h);
+}
+// the product for vectors on the host, or (dev) on this device (PETSc VECCUDA: VecCUDAGetArrayRead /
+// VecCUDAGetArrayWrite, no PCIe traffic); the result is complete when the call returns
+static int mf_apply(int k, const char* who, const double* a, double* y, long long n, double h, bool dev) {
+    const MfOp& op = kMfOps[k];
+    if (op.checkFirst) {
+        if (!a || !y) return fail("%s: null vector", who);
+        if (!op.chooseH && !(h > 0.0)) return fail("%s: h must be positive", who);
+        if (op.check(who, true, n)) return 1;
+    }
+    if (g.mfOwner != k) return fail("%s: %s has not been called", who, op.setBase);
+    const long long need = op.size();
+    if (!a || !y || n != need || (size_t)need > g.nkN) return fail("%s: vector length %lld != local state size %lld", who, n, need);
+    if (dev) {
+        cudaPointerAttributes at;
+        if (cudaPointerGetAttributes(&at, a) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
+            return fail("%s: a is not a device pointer of device %d", who, g.device);
+        if (cudaPointerGetAttributes(&at, y) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != g.device)
+            return fail("%s: y is not a device pointer of device %d", who, g.device);
+    }
+    CK(cudaMemcpyAsync(g.nkA, a, n * sizeof(double), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, g.stream));
+    const int rc = mf_product(k, n, h);
+    if (rc == 1) return 1;
+    if (rc == 0) CK(cudaMemcpyAsync(y, g.nkY, n * sizeof(double), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, g.stream));
+    else if (dev) CK(cudaMemsetAsync(y, 0, n * sizeof(double), g.stream));
+    CK(cudaStreamSynchronize(g.stream));
+    if (rc == 2 && !dev) memset(y, 0, n * sizeof(double));
+    return 0;
+}
+
+int adfb_form_function(const double* wVec, double* rVec, long long n) {
+    ADFB_RANGE("adfb_form_function");
+    NEED_INIT();
+    if (nk_check("adfb_form_function", wVec && rVec, n)) return 1;
+    for (Block& b : g.blocks)
+        if (b.alive && b.level == 1 && !b.haveMetrics) return fail("adfb_form_function: geometry of a block was never set");
+    const int rc = form_function_pipelined(wVec, rVec, n);
+    if (rc >= 0) return rc;
+    return mf_form_function(MF_NK, wVec, rVec, n);
+}
+int adfb_mffd_set_base(const double* U, long long n) {
+    ADFB_RANGE("adfb_mffd_set_base");
+    NEED_INIT();
+    if (nk_check("adfb_mffd_set_base", U != nullptr, n)) return 1;
+    return mf_set_base(MF_NK, U, n);
+}
+int adfb_mffd_apply(const double* a, double* y, long long n, double h) {
+    ADFB_RANGE("adfb_mffd_apply");
+    NEED_INIT();
+    return mf_apply(MF_NK, "adfb_mffd_apply", a, y, n, h, false);
+}
+int adfb_mffd_apply_device(const double* aDev, double* yDev, long long n, double h) {
+    ADFB_RANGE("adfb_mffd_apply_device");
+    NEED_INIT();
+    return mf_apply(MF_NK, "adfb_mffd_apply_device", aDev, yDev, n, h, true);
+}
+double adfb_mffd_last_h(void) { return g.nkLastH; }
+
+int adfb_ank_form_function(const double* inVec, double* rVec, long long n) {
+    ADFB_RANGE("adfb_ank_form_function");
+    NEED_INIT();
+    if (ank_check("adfb_ank_form_function", inVec && rVec, n)) return 1;
+    return mf_form_function(MF_ANK, inVec, rVec, n);
+}
+int adfb_ank_mffd_set_base(const double* U, long long n) {
+    NEED_INIT();
+    if (ank_check("adfb_ank_mffd_set_base", U != nullptr, n)) return 1;
+    return mf_set_base(MF_ANK, U, n);
+}
+int adfb_ank_mffd_apply(const double* a, double* y, long long n, double h) {
+    ADFB_RANGE("adfb_ank_mffd_apply");
+    NEED_INIT();
+    return mf_apply(MF_ANK, "adfb_ank_mffd_apply", a, y, n, h, false);
+}
+int adfb_ank_mffd_apply_device(const double* aDev, double* yDev, long long n, double h) {
+    ADFB_RANGE("adfb_ank_mffd_apply_device");
+    NEED_INIT();
+    return mf_apply(MF_ANK, "adfb_ank_mffd_apply_device", aDev, yDev, n, h, true);
+}
+
+int adfb_ank_form_function_turb(const double* inVec, double* rVec, long long n) {
+    ADFB_RANGE("adfb_ank_form_function_turb");
+    NEED_INIT();
+    if (ank_turb_check("adfb_ank_form_function_turb", inVec && rVec, n)) return 1;
+    return mf_form_function(MF_ANK_TURB, inVec, rVec, n);
+}
 int adfb_ank_mffd_turb_set_base(const double* U, long long n) {
     ADFB_RANGE("adfb_ank_mffd_turb_set_base");
     NEED_INIT();
-    if (!U) return fail("adfb_ank_mffd_turb_set_base: null vector");
-    if (ank_turb_ready("adfb_ank_mffd_turb_set_base", n)) return 1;
-    g.nkHaveBase = false; g.ankHaveBase = false;   // the NK / ANK bases share the buffers
-    CK(cudaMemcpyAsync(g.nkU, U, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (ank_turb_save_dtl()) return 1;
-    if (ank_turb_vec_kernel(g.nkU, nullptr, nullptr, nullptr, 0.0, 0)) return 1;
-    if (adfb_residual(1, ADFB_RES_TURB)) return 1;
-    if (ank_turb_vec_kernel(g.nkU, nullptr, g.nkF0, nullptr, 1.0, 2)) return 1;
-    CK(cudaStreamSynchronize(g.stream));
-    g.ankTurbHaveBase = true;
-    return 0;
+    if (ank_turb_check("adfb_ank_mffd_turb_set_base", U != nullptr, n)) return 1;
+    return mf_set_base(MF_ANK_TURB, U, n);
 }
 int adfb_ank_mffd_turb_apply(const double* a, double* y, long long n, double h) {
     ADFB_RANGE("adfb_ank_mffd_turb_apply");
     NEED_INIT();
-    if (!a || !y) return fail("adfb_ank_mffd_turb_apply: null vector");
-    if (!(h > 0.0)) return fail("adfb_ank_mffd_turb_apply: h must be positive");
-    if (ank_turb_ready("adfb_ank_mffd_turb_apply", n)) return 1;
-    if (!g.ankTurbHaveBase || g.nkHaveBase || g.ankHaveBase) return fail("adfb_ank_mffd_turb_apply: adfb_ank_mffd_turb_set_base has not been called");
-    CK(cudaMemcpyAsync(g.nkA, a, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    if (ank_turb_vec_kernel(g.nkA, g.nkU, nullptr, g.ankPert, h, 1)) return 1;
-    if (adfb_residual(1, ADFB_RES_TURB)) return 1;
-    if (ank_turb_vec_kernel(g.ankPert, g.nkF0, g.nkY, nullptr, h, 3)) return 1;
-    CK(cudaMemcpyAsync(y, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return 0;
+    return mf_apply(MF_ANK_TURB, "adfb_ank_mffd_turb_apply", a, y, n, h, false);
 }
-// physicalityCheckANKTurb (:3212-3335)
-int adfb_ank_physicality_check_turb(const double* wVec, double* deltaW, long long n, double* lambdaP) {
-    ADFB_RANGE("adfb_ank_physicality_check_turb");
-    NEED_INIT();
-    if (!wVec || !deltaW || !lambdaP) return fail("adfb_ank_physicality_check_turb: null argument");
-    if (ank_turb_ready("adfb_ank_physicality_check_turb", n)) return 1;
+
+// physicalityCheckANK (:3013-3210) and physicalityCheckANKTurb (:3212-3335): lambdaP, the fraction of the update deltaW
+// of wVec that keeps the state physical, the minimum over the ranks; the clipped deltaW comes back when copyBack
+static int ank_physicality(bool turb, const double* wVec, double* deltaW, long long n, double* lambdaP, bool copyBack) {
     CK(cudaMemcpyAsync(g.nkA, wVec, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(g.nkY, deltaW, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
     const int nPart = 512;
     KT_BEGIN(K_MFFD, g.stream);
-    k_ank_phys_turb<<<nPart, 256, 0, g.stream>>>(n, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
+    if (turb) {
+        k_ank_phys_turb<<<nPart, 256, 0, g.stream>>>(n, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
+    } else {
+        int ns = 5;
+        for (Block& b : g.blocks) if (b.alive && b.level == 1) { ns = ank_nstate(b); break; }
+        k_ank_phys<<<nPart, 256, 0, g.stream>>>(n / ns, ns, g.ank.coupled, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
+    }
     KT_END(K_MFFD, g.stream);
     KT_BEGIN(K_MFFD, g.stream);
     k_min_final<<<1, 256, 0, g.stream>>>(g.dRed, nPart);
     KT_END(K_MFFD, g.stream);
-    if (g.nranks > 1) {
-        const int rc = g.nccl.AllReduce(g.dRed + nPart, g.dRed + nPart, 1, kNcclDouble, kNcclMin, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, g.dRed + nPart, sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaMemcpyAsync(deltaW, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
+    if (allreduce(g.dRed + nPart, 1, kNcclMin)) return 1;
+    if (copyBack) CK(cudaMemcpyAsync(deltaW, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
+    double lambda = 0.0;
+    if (fetch(g.dRed + nPart, 1, &lambda)) return 1;
     CK(cudaGetLastError());
-    *lambdaP = g.hRed[0];
+    *lambdaP = lambda;
     return 0;
+}
+int adfb_ank_physicality_check_turb(const double* wVec, double* deltaW, long long n, double* lambdaP) {
+    ADFB_RANGE("adfb_ank_physicality_check_turb");
+    NEED_INIT();
+    if (!wVec || !deltaW || !lambdaP) return fail("adfb_ank_physicality_check_turb: null argument");
+    if (ank_turb_check("adfb_ank_physicality_check_turb", true, n)) return 1;
+    return ank_physicality(true, wVec, deltaW, n, lambdaP, true);
 }
 int adfb_ank_physicality_check(const double* wVec, double* deltaW, long long n, double* lambdaP) {
     ADFB_RANGE("adfb_ank_physicality_check");
@@ -1974,27 +1965,7 @@ int adfb_ank_physicality_check(const double* wVec, double* deltaW, long long n, 
     const long long need = ank_vec_size();
     if (n != need) return fail("adfb_ank_physicality_check: vector length %lld != %lld", n, need);
     if (nk_buffers(adfb_state_size())) return 1;
-    CK(cudaMemcpyAsync(g.nkA, wVec, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    CK(cudaMemcpyAsync(g.nkY, deltaW, need * sizeof(double), cudaMemcpyHostToDevice, g.stream));
-    int ns = 5;
-    for (Block& b : g.blocks) if (b.alive && b.level == 1) { ns = ank_nstate(b); break; }
-    const int nPart = 512;
-    KT_BEGIN(K_MFFD, g.stream);
-    k_ank_phys<<<nPart, 256, 0, g.stream>>>(need / ns, ns, g.ank.coupled, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
-    KT_END(K_MFFD, g.stream);
-    KT_BEGIN(K_MFFD, g.stream);
-    k_min_final<<<1, 256, 0, g.stream>>>(g.dRed, nPart);
-    KT_END(K_MFFD, g.stream);
-    if (g.nranks > 1) {
-        const int rc = g.nccl.AllReduce(g.dRed + nPart, g.dRed + nPart, 1, kNcclDouble, kNcclMin, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, g.dRed + nPart, sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    if (g.ank.coupled) CK(cudaMemcpyAsync(deltaW, g.nkY, need * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    CK(cudaGetLastError());
-    *lambdaP = g.hRed[0];
-    return 0;
+    return ank_physicality(false, wVec, deltaW, n, lambdaP, g.ank.coupled);
 }
 
 // ---------------------------------------------------------------------------
@@ -2287,9 +2258,9 @@ int adfb_mg_cycle(int nSteps, const int* cycling, int smoother) {
 // the assembled approximate Jacobian in the reference) stays outside: pc == NULL is the identity, otherwise
 // pc(ctx, inDev, outDev, n) applies M^-1 to a device vector.
 static int kry_apply_op(int op, const double* inDev, double* outDev, long long n) {
-    if (op == 2) return ank_vec_kernel(inDev, nullptr, outDev, nullptr, 1.0, 4);   // y = timeStepMat x (linear)
+    if (op == 2) return ank_vec_kernel(4, inDev, nullptr, outDev, 1.0);   // y = timeStepMat x (linear)
     CK(cudaMemcpyAsync(g.nkA, inDev, n * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
-    const int rc = op == 0 ? mffd_core(n, -1.0) : ank_mffd_core(n, -1.0);
+    const int rc = mf_product(op == 0 ? MF_NK : MF_ANK, n, -1.0);
     if (rc == 1) return 1;
     if (rc == 2) CK(cudaMemsetAsync(outDev, 0, n * sizeof(double), g.stream));
     else CK(cudaMemcpyAsync(outDev, g.nkY, n * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
@@ -2303,14 +2274,7 @@ static int kry_dots(const double* V, long long ld, int nv, const double* w, long
     KT_BEGIN(K_MFFD, g.stream);
     k_multidot_final<<<nv, 256, 0, g.stream>>>(g.kryRed, ADFB_GMRES_PARTS, nv, fin);
     KT_END(K_MFFD, g.stream);
-    if (g.nranks > 1) {
-        const int rc = g.nccl.AllReduce(fin, fin, nv, kNcclDouble, kNcclSum, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, fin, nv * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    for (int i = 0; i < nv; i++) hOut[i] = g.hRed[i];
-    return 0;
+    return allreduce_fetch(fin, nv, kNcclSum, hOut);
 }
 int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int restart, int maxIts, double rtol, double atol,
                      AdfbPrecondFn pc, void* pcCtx, int* itsOut, double* resNormOut) {
@@ -2320,15 +2284,12 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
     if (op < 0 || op > 2) return fail("adfb_gmres_solve: op must be 0 (NK product), 1 (ANK product) or 2 (time-step matrix)");
     if (restart < 1 || restart > ADFB_GMRES_MAXV - 2) return fail("adfb_gmres_solve: restart must be in 1..%d", ADFB_GMRES_MAXV - 2);
     if (maxIts < 1) return fail("adfb_gmres_solve: maxIts must be >= 1");
-    long long need = 0;
-    if (op == 0) {
-        if (!g.nkHaveBase) return fail("adfb_gmres_solve: adfb_mffd_set_base has not been called");
-        need = adfb_state_size();
-    } else {
-        if (ank_ready("adfb_gmres_solve", n, &need)) return 1;
-        if (op == 1 && !g.ankHaveBase) return fail("adfb_gmres_solve: adfb_ank_mffd_set_base has not been called");
-    }
-    if (n != need) return fail("adfb_gmres_solve: vector length %lld != %lld", n, need);
+    const int k = op == 0 ? MF_NK : MF_ANK;   // op 2 needs the ANK operator ready, not its base
+    const MfOp& mf = kMfOps[k];
+    if (mf.checkFirst && mf.check("adfb_gmres_solve", true, n)) return 1;
+    if (op < 2 && g.mfOwner != k) return fail("adfb_gmres_solve: %s has not been called", mf.setBase);
+    const long long need = mf.size();
+    if (n != need || (size_t)need > g.nkN) return fail("adfb_gmres_solve: vector length %lld != %lld", n, need);
     const int m = restart;
     const size_t nvec = (size_t)m + 4;   // V_0..V_m, w, z, xDev
     if (g.kryVN < nvec * (size_t)n) {
@@ -2465,15 +2426,10 @@ static int monitor_impl(int level, unsigned what, double out[ADFB_MON_N]) {
         bi++;
     }
     if (launch_norms_final(g.dMon, nPart, stride, nBlk, what, mc.hInf, res, g.stream)) return fail("monitor kernel failed");
-    if (g.nranks > 1) {   // mpi_allreduce of monLoc: the sums with mpi_sum, the maxima with mpi_max (solvers.F90:1537-1545)
-        int rc = g.nccl.AllReduce(res, res, ADFB_MON_NSUM, kNcclDouble, kNcclSum, g.comm, g.stream);
-        if (rc == 0) rc = g.nccl.AllReduce(res + ADFB_MON_NSUM, res + ADFB_MON_NSUM, ADFB_MON_N - ADFB_MON_NSUM, kNcclDouble, kNcclMax, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, res, ADFB_MON_N * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    for (int v = 0; v < ADFB_MON_N; v++) out[v] = g.hRed[v];
-    return 0;
+    // mpi_allreduce of monLoc: the sums with mpi_sum, the maxima with mpi_max (solvers.F90:1537-1545)
+    if (allreduce(res, ADFB_MON_NSUM, kNcclSum)) return 1;
+    if (allreduce(res + ADFB_MON_NSUM, ADFB_MON_N - ADFB_MON_NSUM, kNcclMax)) return 1;
+    return fetch(res, ADFB_MON_N, out);
 }
 
 int adfb_monitor(int level, unsigned what, double out[10]) {
@@ -2631,24 +2587,12 @@ int adfb_forces(int level, const double refPoint[3], double pRef, double out[12]
     ADFB_RANGE("adfb_forces");
     NEED_INIT();
     if (!refPoint || !out) return fail("adfb_forces: null");
-    if (g.dRedN < 16) {
-        if (g.dRed) cudaFree(g.dRed);
-        CK(cudaMalloc((void**)&g.dRed, 2050 * sizeof(double)));
-        g.dRedN = 2050;
-    }
     CK(cudaMemsetAsync(g.dRed, 0, 12 * sizeof(double), g.stream));
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
         if (launch_wall_forces(b.d, b.dev, b.subfaces, refPoint, pRef, g.dRed, g.stream)) return fail("force kernel failed");
     }
-    if (g.nranks > 1) {
-        const int rc = g.nccl.AllReduce(g.dRed, g.dRed, 12, kNcclDouble, kNcclSum, g.comm, g.stream);
-        if (rc != 0) return fail("ncclAllReduce: %s", g.nccl.GetErrorString(rc));
-    }
-    CK(cudaMemcpyAsync(g.hRed, g.dRed, 12 * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    for (int q = 0; q < 12; q++) out[q] = g.hRed[q];
-    return 0;
+    return allreduce_fetch(g.dRed, 12, kNcclSum, out);
 }
 
 }  // extern "C"
