@@ -2311,12 +2311,15 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
     double bb = 0.0;
     if (kry_dots(w, n, 1, w, n, &bb)) return 1;
     const double bnorm = sqrt(bb);
-    double rnorm = bnorm;
+    // A non-finite ||b||, projection, column norm, rotation, restart residual or update of x ends the solve with resNorm =
+    // NaN, as the reference's KSP ends such a solve as diverged and leaves the NaN to the caller's convergence check.
+    bool stop = !std::isfinite(bnorm);
+    double rnorm = stop ? NAN : bnorm;
     const double target = fmax(rtol * bnorm, atol);
     int its = 0;
     std::vector<double> H((size_t)(m + 1) * m), cs(m), sn(m), gg(m + 1), hcol(m + 2);
     bool first = true;
-    while (its < maxIts && rnorm > target) {
+    while (!stop && its < maxIts && rnorm > target) {
         if (!first) {   // restart: r = b - A M^-1 ... with right preconditioning x already holds M^-1 (V y): r = b - A x
             if (kry_apply_op(op, xd, w, n)) return 1;
             CK(cudaMemcpyAsync(z, rhs, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
@@ -2324,6 +2327,7 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
             k_axpy_many<<<nb, 256, 0, g.stream>>>(z, n, 1, c1, -1.0, w, n);   // w = -w + b
             if (kry_dots(w, n, 1, w, n, &bb)) return 1;
             rnorm = sqrt(bb);
+            if (!std::isfinite(rnorm)) { rnorm = NAN; break; }
             if (rnorm <= target) break;
         }
         first = false;
@@ -2348,6 +2352,9 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
             double ww = 0.0;
             if (kry_dots(w, n, 1, w, n, &ww)) return 1;
             hcol[j + 1] = sqrt(ww);
+            bool finite = std::isfinite(hcol[j + 1]);
+            for (int i = 0; i <= j; i++) finite = finite && std::isfinite(hcol[i]);
+            if (!finite) { its++; rnorm = NAN; stop = true; break; }
             if (hcol[j + 1] > 0.0) k_scale_to<<<nb, 256, 0, g.stream>>>(w, 1.0 / hcol[j + 1], V + (size_t)(j + 1) * n, n);
             // Givens rotations on the new column
             for (int i = 0; i < j; i++) {
@@ -2356,19 +2363,24 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
                 hcol[i] = t;
             }
             const double den = hypot(hcol[j], hcol[j + 1]);
-            cs[j] = den > 0.0 ? hcol[j] / den : 1.0;
-            sn[j] = den > 0.0 ? hcol[j + 1] / den : 0.0;
+            if (!std::isfinite(den)) { its++; rnorm = NAN; stop = true; break; }
+            // exact breakdown with a zero column: A M^-1 v_j adds nothing to the span, now or after any restart, so the
+            // solve ends with the first j columns and the residual they leave, |g_j|
+            if (den == 0.0) { its++; rnorm = fabs(gg[j]); stop = true; break; }
+            cs[j] = hcol[j] / den;
+            sn[j] = hcol[j + 1] / den;
             hcol[j] = den;
             gg[j + 1] = -sn[j] * gg[j];
             gg[j] = cs[j] * gg[j];
             for (int i = 0; i <= j; i++) H[(size_t)i + (size_t)(m + 1) * j] = hcol[i];
             its++;
             rnorm = fabs(gg[j + 1]);
-            if (den == 0.0) break;   // exact breakdown with a zero column: solve with the first j columns only
             if (rnorm <= target) { j++; break; }
         }
+        if (std::isnan(rnorm)) break;
         // y = H^-1 g (upper triangular), x += M^-1 (V y)
         const int k = j;
+        if (k == 0) break;
         std::vector<double> y(k);
         for (int i = k - 1; i >= 0; i--) {
             double t = gg[i];
@@ -2388,6 +2400,11 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
         } else {
             k_axpy_many<<<nb, 256, 0, g.stream>>>(V, n, k, cy, 1.0, xd, n);
         }
+    }
+    if (its > 0 && !std::isnan(rnorm)) {   // a non-finite update (the callback's, or an overflowing y) reports NaN as well
+        double xx = 0.0;
+        if (kry_dots(xd, n, 1, xd, n, &xx)) return 1;
+        if (!std::isfinite(xx)) rnorm = NAN;
     }
     CK(cudaMemcpyAsync(x, xd, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));

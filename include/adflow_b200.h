@@ -422,7 +422,13 @@ int adfb_ank_physicality_check(const double* wVec, double* deltaW, long long n, 
    (adfb_ank_time_step_mat + adfb_ank_mffd_set_base first), op 2: the block-diagonal time-step matrix alone (a linear
    operator; used to verify the solver).  pc == NULL: identity; otherwise pc(ctx, inDev, outDev, n) applies
    the right preconditioner M^-1 to a DEVICE vector (the reference's ASM/ILU of the assembled approximate Jacobian stays
-   with PETSc).  rhs, x: host vectors; its / resNorm (||b - A x|| estimate) may be NULL. */
+   with PETSc).  rhs, x: host vectors; its / resNorm (||b - A x|| estimate) may be NULL.
+   Stopping: its is the first step whose residual meets max(rtol ||b||, atol) (0 when ||b|| does), or maxIts.
+   A non-finite ||b||, projection, Arnoldi column norm, rotation, restart residual or update of x ends the solve: it
+   returns 0 with the steps taken counted in its and resNorm = NaN, for the caller's convergence check to see, and x is
+   not to be used.  An exact breakdown with a zero column (A M^-1 v_j in the span of the previous products: a singular
+   operator, or a preconditioner with a null space) also ends it, with x from the first j Krylov vectors and resNorm
+   the residual they leave, which no further step or restart could reduce. */
 typedef int (*AdfbPrecondFn)(void* ctx, const double* inDev, double* outDev, long long n);
 int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int restart, int maxIts, double rtol, double atol,
                      AdfbPrecondFn pc, void* pcCtx, int* its, double* resNorm);
