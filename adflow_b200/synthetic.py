@@ -320,13 +320,14 @@ def mg_tables_1d(keep, ie_c, ie_f, ib_f):
     return fine, wgt, coarse
 
 
-def make_coarse_block(fine, prm):
+def make_coarse_block(fine, prm, keeps=None):
     """The next coarser level of `fine`: nodes = the kept fine nodes (halo nodes extrapolated), metrics, volumes,
     wall distance (volume average), porosities and boundary subfaces of the same types, restriction tables on the
     coarse block and interpolation tables on `fine` (fine.mg is updated).  The state is left zero: it is the
-    output of the restriction."""
+    output of the restriction.  keeps: iCo, jCo, kCo (as mg_kept_nodes returns them); default mg_kept_nodes."""
     df = fine.d
-    keeps = [mg_kept_nodes(n) for n in (df.nx, df.ny, df.nz)]
+    if keeps is None:
+        keeps = [mg_kept_nodes(n) for n in (df.nx, df.ny, df.nz)]
     nc = [int(k.sum()) - 1 for k in keeps]
     blk = HostBlock(*nc, nw=fine.nw, right_handed=fine.right_handed)
     blk.level = fine.level + 1
