@@ -178,9 +178,6 @@ static inline int adfb_part_lanes(int nl) {
     if (nl > 128 && nl <= 256) return 16;
     return 0;
 }
-// every launch site sits in an NVTX range named after its kernel family (SURVEY section 5: tracing)
-#define KT_BEGIN(id, stream) do { nvtxRangePushA(kKernelNames[id]); g_kt.begin(id, stream); } while (0)
-#define KT_END(id, stream) do { g_kt.end(id, stream); nvtxRangePop(); } while (0)
 struct AdfbRange {   // NVTX range of one C-ABI entry point
     explicit AdfbRange(const char* name) { nvtxRangePushA(name); }
     ~AdfbRange() { nvtxRangePop(); }
@@ -188,18 +185,28 @@ struct AdfbRange {   // NVTX range of one C-ABI entry point
 #define ADFB_RANGE(name) AdfbRange adfb_range_(name)
 
 // ---------------------------------------------------------------------------
-// Launch with the programmatic-dependent-launch attribute (the kernel must call
-// cudaGridDependencySynchronize() before touching memory).  ADFB_PDL=0 falls back to a plain launch.
+// Every kernel launch of the library goes through launch_kernel: one launch of `kern`, in an NVTX range named after its
+// family `fam` (SURVEY section 5: tracing), counted once in g_kt (adfb_launch_count, the graph cache's per-graph count)
+// and, with timing on, between the family's event pair.  With `pdl` the launch carries the programmatic-dependent-launch
+// attribute, so `kern` must open with ADFB_PDL_SYNC() before touching memory; ADFB_PDL=0 drops the attribute from every
+// launch.  Returns the launch's error.
+static bool pdl_enabled() {
+    static const bool on = [] { const char* e = getenv("ADFB_PDL"); return e ? atoi(e) != 0 : true; }();
+    return on;
+}
 template <typename... KArgs, typename... Args>
-static void launch_pdl(void (*kern)(KArgs...), dim3 g, dim3 tb, cudaStream_t s, Args... args) {
-    static int pdl = -1;
-    if (pdl < 0) { const char* e = getenv("ADFB_PDL"); pdl = e ? atoi(e) : 1; }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = g; cfg.blockDim = tb; cfg.dynamicSmemBytes = 0; cfg.stream = s;
+static cudaError_t launch_kernel(KernelId fam, bool pdl, dim3 grid, dim3 block, size_t smem, cudaStream_t s, void (*kern)(KArgs...),
+                                 Args... args) {
+    nvtxRangePushA(kKernelNames[fam]);
+    g_kt.begin(fam, s);
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.attrs = attr; cfg.numAttrs = (pdl && pdl_enabled()) ? 1 : 0;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+    g_kt.end(fam, s);
+    nvtxRangePop();
+    return e;
 }
-

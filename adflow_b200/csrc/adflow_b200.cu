@@ -493,6 +493,8 @@ int adfb_synchronize(void) {
     return 0;
 }
 
+// one count per kernel launch (launch_kernel), a launch recorded while a CUDA graph is captured included, and a graph's
+// count each time it is replayed
 long long adfb_launch_count(void) { return g_kt.launches; }
 int adfb_graph_count(void) { return g.useGraphs ? (int)g.graphs.size() : -1; }
 /* per-kernel CUDA-event timing (bench.py roofline pass): on=1 starts recording and
@@ -538,7 +540,7 @@ int adfb_set_params(const AdfbParams* prm) {
         fheat[7] = 1.0 / gm1; fheat[8] = 0.000001 * g.prm.gammaInf * g.prm.pInfCorr / g.prm.rhoInf;
         diss_coefs(fheat + 9);
         CK(cudaMemcpyToSymbolAsync(c_fheat, fheat, sizeof fheat, 0, cudaMemcpyHostToDevice, g.stream));
-        k_param_consts<<<1, 1, 0, g.stream>>>(g.dConst);   // reads the c_prm uploaded above (stream order)
+        launch_kernel(K_MISC, false, 1, 1, 0, g.stream, k_param_consts, g.dConst);   // reads the c_prm uploaded above (stream order)
         CK(cudaMemcpyToSymbolAsync(c_fheat, g.dConst, sizeof(double), 2 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
         CK(cudaMemcpyToSymbolAsync(c_fheat, g.dConst + 1, 2 * sizeof(double), 5 * sizeof(double), cudaMemcpyDeviceToDevice, g.stream));
         CK(cudaStreamSynchronize(g.stream));
@@ -1014,13 +1016,12 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
         }
         if (doPost && P.nSend) {
             const long long n = P.nSend * nVar;
-            KT_BEGIN(K_HALO, cs);
             if (P.interp)
-                k_halo_pack_interp<<<(unsigned)((n + 255) / 256), 256, 0, cs>>>(P.sBlk, P.sOff, P.sCum, P.sLocal, P.sCount, P.sSJ, P.sSK,
-                                                                               P.sW, dTab, nVar, P.nSend, P.sendBuf);
+                launch_kernel(K_HALO, false, (unsigned)((n + 255) / 256), 256, 0, cs, k_halo_pack_interp, P.sBlk, P.sOff, P.sCum, P.sLocal, P.sCount,
+                              P.sSJ, P.sSK, P.sW, dTab, nVar, P.nSend, P.sendBuf);
             else
-                k_halo_pack<<<(unsigned)((n + 255) / 256), 256, 0, cs>>>(P.sBlk, P.sOff, P.sCum, P.sLocal, P.sCount, dTab, nVar, P.nSend, P.sendBuf);
-            KT_END(K_HALO, cs);
+                launch_kernel(K_HALO, false, (unsigned)((n + 255) / 256), 256, 0, cs, k_halo_pack, P.sBlk, P.sOff, P.sCum, P.sLocal, P.sCount, dTab,
+                              nVar, P.nSend, P.sendBuf);
         }
         if (doPost && !P.nbrRank.empty()) {
             int rc = g.nccl.GroupStart();
@@ -1038,19 +1039,17 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
         if (!doFinish) continue;
         if (P.nInt) {
             const long long n = P.nInt * nVar;
-            KT_BEGIN(K_HALO, g.stream);
             if (P.interp)
-                k_halo_internal_interp<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(P.iSrcBlk, P.iSrcOff, P.iSJ, P.iSK, P.iW, P.iDstBlk,
-                                                                                         P.iDstOff, dTab, nVar, P.nInt);
+                launch_kernel(K_HALO, false, (unsigned)((n + 255) / 256), 256, 0, g.stream, k_halo_internal_interp, P.iSrcBlk, P.iSrcOff, P.iSJ,
+                              P.iSK, P.iW, P.iDstBlk, P.iDstOff, dTab, nVar, P.nInt);
             else
-                k_halo_internal<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(P.iSrcBlk, P.iSrcOff, P.iDstBlk, P.iDstOff, dTab, nVar, P.nInt);
-            KT_END(K_HALO, g.stream);
+                launch_kernel(K_HALO, false, (unsigned)((n + 255) / 256), 256, 0, g.stream, k_halo_internal, P.iSrcBlk, P.iSrcOff, P.iDstBlk,
+                              P.iDstOff, dTab, nVar, P.nInt);
         }
         if (P.nRecv) {
             const long long n = P.nRecv * nVar;
-            KT_BEGIN(K_HALO, g.stream);
-            k_halo_unpack<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(P.rBlk, P.rOff, P.rCum, P.rLocal, P.rCount, dTab, nVar, P.nRecv, P.recvBuf);
-            KT_END(K_HALO, g.stream);
+            launch_kernel(K_HALO, false, (unsigned)((n + 255) / 256), 256, 0, g.stream, k_halo_unpack, P.rBlk, P.rOff, P.rCum, P.rLocal, P.rCount,
+                          dTab, nVar, P.nRecv, P.recvBuf);
         }
     }
     // orphanAverage on every block that carries an orphan list (haloExchange.F90:56-66, :161-171)
@@ -1058,11 +1057,8 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
         for (Block& b : g.blocks) {
             if (!b.alive || b.level != level || b.nOrphans == 0) continue;
             const int lEnd = end < b.nw ? end : b.nw;
-            KT_BEGIN(K_HALO, g.stream);
-            k_orphan_average<<<(b.nOrphans + 127) / 128, 128, 0, g.stream>>>(b.d, b.dev, b.nOrphans, b.dOrphans, start, lEnd, commPressure ? 1 : 0,
-                                                                             (viscous && commViscous) ? 1 : 0, (eddy && commViscous) ? 1 : 0,
-                                                                             b.muInf, b.eddyVisInfRatio);
-            KT_END(K_HALO, g.stream);
+            launch_kernel(K_HALO, false, (b.nOrphans + 127) / 128, 128, 0, g.stream, k_orphan_average, b.d, b.dev, b.nOrphans, b.dOrphans, start,
+                          lEnd, commPressure ? 1 : 0, (viscous && commViscous) ? 1 : 0, (eddy && commViscous) ? 1 : 0, b.muInf, b.eddyVisInfRatio);
         }
     }
     // bothPAndE: computeEtotBlock(2, il, 2, jl, 2, kl) on every block (haloExchange.F90:174-197)
@@ -1071,9 +1067,7 @@ static int halo_exchange_impl(int level, int start, int end, int commPressure, i
             if (!b.alive || b.level != level) continue;
             dim3 tb(32, 4, 2);
             dim3 gr((b.d.nx + 31) / 32, (b.d.ny + 3) / 4, (b.d.nz + 1) / 2);
-            KT_BEGIN(K_HALO, g.stream);
-            k_etot_owned<<<gr, tb, 0, g.stream>>>(b.d, b.dev);
-            KT_END(K_HALO, g.stream);
+            launch_kernel(K_HALO, false, gr, tb, 0, g.stream, k_etot_owned, b.d, b.dev);
         }
     }
     CK(cudaGetLastError());
@@ -1171,10 +1165,8 @@ static int nk_vec_kernel(int mode, const double* vec, const double* base, double
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
         const long long n = (long long)b.d.nx * b.d.ny * b.d.nz * b.nw;
-        KT_BEGIN(K_MFFD, g.stream);
-        k_nkvec<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, b.nw, vec ? vec + off : nullptr, base ? base + off : nullptr,
-                                                                   out ? out + off : nullptr, h, mode, 0LL, LLONG_MAX);
-        KT_END(K_MFFD, g.stream);
+        launch_kernel(K_MFFD, false, (unsigned)((n + 255) / 256), 256, 0, g.stream, k_nkvec, b.d, b.dev, b.nw, vec ? vec + off : nullptr,
+                      base ? base + off : nullptr, out ? out + off : nullptr, h, mode, 0LL, LLONG_MAX);
         off += n;
     }
     CK(cudaGetLastError());
@@ -1183,12 +1175,8 @@ static int nk_vec_kernel(int mode, const double* vec, const double* base, double
 // sum of squares of a device vector, all-reduced; result in *out
 static int nk_sumsq(const double* v, long long n, double* out) {
     const int nPart = 512;
-    KT_BEGIN(K_MFFD, g.stream);
-    k_sumsq_partial<<<nPart, 256, 0, g.stream>>>(v, n, g.dRed);
-    KT_END(K_MFFD, g.stream);
-    KT_BEGIN(K_MFFD, g.stream);
-    k_sum_final<<<1, 256, 0, g.stream>>>(g.dRed, nPart);
-    KT_END(K_MFFD, g.stream);
+    launch_kernel(K_MFFD, false, nPart, 256, 0, g.stream, k_sumsq_partial, v, n, g.dRed);
+    launch_kernel(K_MFFD, false, 1, 256, 0, g.stream, k_sum_final, g.dRed, nPart);
     return allreduce_fetch(g.dRed + nPart, 1, kNcclSum, out);
 }
 static const unsigned kNkFlags = ADFB_RES_FLOW | ADFB_RES_TURB;
@@ -1261,14 +1249,10 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
             // setW + p / rlv / rev of the slab's owned cells
             {
                 const long long q0 = (long long)o0 * plane, q1 = (long long)o1 * plane;
-                KT_BEGIN(K_MFFD, sF);
-                k_nkvec<<<(unsigned)((q1 - q0 + 255) / 256), 256, 0, sF>>>(d, b.dev, b.nw, g.nkA + off, nullptr, nullptr, 0.0, 0, q0, q1);
-                KT_END(K_MFFD, sF);
+                launch_kernel(K_MFFD, false, (unsigned)((q1 - q0 + 255) / 256), 256, 0, sF, k_nkvec, d, b.dev, b.nw, g.nkA + off, nullptr, nullptr, 0.0, 0, q0, q1);
                 dim3 tb(32, 4, 2);
                 dim3 gr((d.nx + 31) / 32, (d.ny + 3) / 4, (o1 - o0 + 1) / 2);
-                KT_BEGIN(K_STATE, sF);
-                launch_pdl(k_state_prep, gr, tb, sF, d, b.dev, 0, rans ? 6 : 5, 1, o0, 1 + o1);
-                KT_END(K_STATE, sF);
+                launch_kernel(K_STATE, true, gr, tb, 0, sF, k_state_prep, d, b.dev, 0, rans ? 6 : 5, 1, o0, 1 + o1);
             }
             // boundary conditions of the slab's planes (+ the k-face subfaces with the first / last slab)
             const int pLo = first ? 0 : 2 + o0, pHi = last ? d.kb : 1 + o1;
@@ -1279,9 +1263,7 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
             {
                 dim3 tb(32, 4, 2);
                 dim3 gr((d.NI + 31) / 32, (d.NJ + 3) / 4, (pHi - pLo + 2) / 2);
-                KT_BEGIN(K_PREP, sF);
-                launch_pdl(k_prep, gr, tb, sF, d, b.dev, 1, 1, pLo, pHi, residual_discr(1, true), 1);
-                KT_END(K_PREP, sF);
+                launch_kernel(K_PREP, true, gr, tb, 0, sF, k_prep, d, b.dev, 1, 1, pLo, pHi, residual_discr(1, true), 1);
             }
             // residual rows of the k chunks whose +-2 plane stencil is complete
             int cEnd = cNext;
@@ -1291,20 +1273,14 @@ static int form_function_pipe_body(const double* wVec, double* rVec, int wantSla
                 CK(cudaStreamWaitEvent(sB, g.ffEv[2][q], 0));
                 const int r0 = ownedEnd(cNext), r1 = ownedEnd(cEnd);
                 if (rans) {
-                    KT_BEGIN(K_SA, sB);
-                    const int rcSa = launch_sa(d, b.dev, g.env, MffdEpi{nullptr, 0}, r0, 1 + r1, sB);
-                    KT_END(K_SA, sB);
-                    if (rcSa) return fail("SA row launch failed inside the form-function pipeline");
+                    if (launch_sa(d, b.dev, g.env, MffdEpi{nullptr, 0}, r0, 1 + r1, sB))
+                        return fail("SA row launch failed inside the form-function pipeline");
                 }
-                KT_BEGIN(K_RESID, sB);
                 const int rc = launch_flowres_tile(d, b.dev, g.prm, g.env, (int)((b.dev.p - b.dev.w) / d.N), 1.0, 1, true, 0, sB, MffdEpi{nullptr, 0},
                                                    kc, cNext, cEnd - cNext);
-                KT_END(K_RESID, sB);
                 if (rc) return fail("tile kernel launch failed inside the form-function pipeline");
                 const long long q0 = (long long)r0 * plane, q1 = (long long)r1 * plane;
-                KT_BEGIN(K_MFFD, sB);
-                k_nkvec<<<(unsigned)((q1 - q0 + 255) / 256), 256, 0, sB>>>(d, b.dev, b.nw, nullptr, nullptr, g.nkY + off, 1.0, 2, q0, q1);
-                KT_END(K_MFFD, sB);
+                launch_kernel(K_MFFD, false, (unsigned)((q1 - q0 + 255) / 256), 256, 0, sB, k_nkvec, d, b.dev, b.nw, nullptr, nullptr, g.nkY + off, 1.0, 2, q0, q1);
                 CK(cudaEventRecord(g.ffEv[1][q], sB));
                 CK(cudaStreamWaitEvent(g.ffOut, g.ffEv[1][q], 0));
                 CK(cudaMemcpyAsync(rVec + off + q0, g.nkY + off + q0, (size_t)(q1 - q0) * sizeof(double), cudaMemcpyDeviceToHost, g.ffOut));
@@ -1398,9 +1374,7 @@ static int nk_mffd_fused(double h) {
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
         const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz;
-        KT_BEGIN(K_MFFD, g.stream);
-        k_nkvec_prep<<<(unsigned)((nc + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, b.nw, g.nkA + off, g.nkU + off, g.dMffd, 1);
-        KT_END(K_MFFD, g.stream);
+        launch_kernel(K_MFFD, false, (unsigned)((nc + 255) / 256), 256, 0, g.stream, k_nkvec_prep, b.d, b.dev, b.nw, g.nkA + off, g.nkU + off, g.dMffd, 1);
         off += nc * b.nw;
     }
     g.mffdFuse = true;
@@ -1415,9 +1389,7 @@ int adfb_reference_shock_sensor(int level) {
     if (!g.havePrm) return fail("adfb_reference_shock_sensor: adfb_set_params has not been called");
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != level) continue;
-        KT_BEGIN(K_MISC, g.stream);
-        k_shock<<<(unsigned)((b.d.N + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, residual_discr(level, true));
-        KT_END(K_MISC, g.stream);
+        launch_kernel(K_MISC, false, (unsigned)((b.d.N + 255) / 256), 256, 0, g.stream, k_shock, b.d, b.dev, residual_discr(level, true));
     }
     CK(cudaGetLastError());
     return 0;
@@ -1452,9 +1424,7 @@ int adfb_timestep(int level, int onlyRadii) {
         if (!b.alive || b.level != level) continue;
         dim3 tb(32, 4, 2);
         dim3 gr((b.d.NI + 31) / 32, (b.d.NJ + 3) / 4, (b.d.NK + 1) / 2);
-        KT_BEGIN(K_PREP, g.stream);
-        launch_pdl(k_prep, gr, tb, g.stream, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, INT_MAX, residual_discr(level, false), scaleRad);
-        KT_END(K_PREP, g.stream);
+        launch_kernel(K_PREP, true, gr, tb, 0, g.stream, k_prep, b.d, b.dev, onlyRadii ? 0 : 1, 1, 0, INT_MAX, residual_discr(level, false), scaleRad);
     }
     CK(cudaGetLastError());
     return 0;
@@ -1653,10 +1623,8 @@ int adfb_ank_time_step_mat(void) {
         if (!b.alive || b.level != 1) continue;
         const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz;
         const int ns = ank_nstate(b);
-        KT_BEGIN(K_MFFD, g.stream);
-        if (ns == 5) k_ank_tsblock<5><<<(unsigned)((nc + 63) / 64), 64, 0, g.stream>>>(b.d, b.dev, g.ank, g.ankT + off);
-        else k_ank_tsblock<6><<<(unsigned)((nc + 63) / 64), 64, 0, g.stream>>>(b.d, b.dev, g.ank, g.ankT + off);
-        KT_END(K_MFFD, g.stream);
+        if (ns == 5) launch_kernel(K_MFFD, false, (unsigned)((nc + 63) / 64), 64, 0, g.stream, k_ank_tsblock<5>, b.d, b.dev, g.ank, g.ankT + off);
+        else launch_kernel(K_MFFD, false, (unsigned)((nc + 63) / 64), 64, 0, g.stream, k_ank_tsblock<6>, b.d, b.dev, g.ank, g.ankT + off);
         off += (size_t)nc * ns * ns;
     }
     CK(cudaGetLastError());
@@ -1673,11 +1641,8 @@ static int ank_vec_kernel(int mode, const double* vec, const double* base, doubl
         if (!b.alive || b.level != 1) continue;
         const int ns = ank_nstate(b);
         const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz, n = nc * ns;
-        KT_BEGIN(K_MFFD, g.stream);
-        k_ankvec<<<(unsigned)((n + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, ns, vec ? vec + off : nullptr, base ? base + off : nullptr,
-                                                                    out ? out + off : nullptr, pert ? pert + off : nullptr,
-                                                                    g.ankT ? g.ankT + offT : nullptr, h, mode);
-        KT_END(K_MFFD, g.stream);
+        launch_kernel(K_MFFD, false, (unsigned)((n + 255) / 256), 256, 0, g.stream, k_ankvec, b.d, b.dev, ns, vec ? vec + off : nullptr,
+                      base ? base + off : nullptr, out ? out + off : nullptr, pert ? pert + off : nullptr, g.ankT ? g.ankT + offT : nullptr, h, mode);
         off += n;
         offT += (size_t)nc * ns * ns;
     }
@@ -1735,10 +1700,8 @@ static int ank_turb_vec_kernel(int mode, const double* vec, const double* base, 
     for (Block& b : g.blocks) {
         if (!b.alive || b.level != 1) continue;
         const long long nc = (long long)b.d.nx * b.d.ny * b.d.nz;
-        KT_BEGIN(K_MFFD, g.stream);
-        k_ankvec_turb<<<(unsigned)((nc + 255) / 256), 256, 0, g.stream>>>(b.d, b.dev, g.ank, b.dev.scratch, vec ? vec + off : nullptr, base ? base + off : nullptr,
-                                                                         out ? out + off : nullptr, pert ? pert + off : nullptr, h, mode);
-        KT_END(K_MFFD, g.stream);
+        launch_kernel(K_MFFD, false, (unsigned)((nc + 255) / 256), 256, 0, g.stream, k_ankvec_turb, b.d, b.dev, g.ank, b.dev.scratch,
+                      vec ? vec + off : nullptr, base ? base + off : nullptr, out ? out + off : nullptr, pert ? pert + off : nullptr, h, mode);
         off += nc;
     }
     CK(cudaGetLastError());
@@ -1930,18 +1893,14 @@ static int ank_physicality(bool turb, const double* wVec, double* deltaW, long l
     CK(cudaMemcpyAsync(g.nkA, wVec, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(g.nkY, deltaW, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
     const int nPart = 512;
-    KT_BEGIN(K_MFFD, g.stream);
     if (turb) {
-        k_ank_phys_turb<<<nPart, 256, 0, g.stream>>>(n, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
+        launch_kernel(K_MFFD, false, nPart, 256, 0, g.stream, k_ank_phys_turb, n, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
     } else {
         int ns = 5;
         for (Block& b : g.blocks) if (b.alive && b.level == 1) { ns = ank_nstate(b); break; }
-        k_ank_phys<<<nPart, 256, 0, g.stream>>>(n / ns, ns, g.ank.coupled, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
+        launch_kernel(K_MFFD, false, nPart, 256, 0, g.stream, k_ank_phys, n / ns, ns, g.ank.coupled, g.ank, g.nkA, g.nkY, *lambdaP, g.dRed);
     }
-    KT_END(K_MFFD, g.stream);
-    KT_BEGIN(K_MFFD, g.stream);
-    k_min_final<<<1, 256, 0, g.stream>>>(g.dRed, nPart);
-    KT_END(K_MFFD, g.stream);
+    launch_kernel(K_MFFD, false, 1, 256, 0, g.stream, k_min_final, g.dRed, nPart);
     if (allreduce(g.dRed + nPart, 1, kNcclMin)) return 1;
     if (copyBack) CK(cudaMemcpyAsync(deltaW, g.nkY, n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
     double lambda = 0.0;
@@ -1973,9 +1932,7 @@ int adfb_ank_physicality_check(const double* wVec, double* deltaW, long long n, 
 static void launch_mg_cells1(const Dims& d, const BlockDev& b, int mode, cudaStream_t s) {
     dim3 tb(32, 4, 2);
     dim3 gr((d.ie + 31) / 32, (d.je + 3) / 4, (d.ke + 1) / 2);
-    KT_BEGIN(K_MISC, s);
-    launch_pdl(k_mg_cells1, gr, tb, s, d, b, mode);
-    KT_END(K_MISC, s);
+    launch_kernel(K_MISC, true, gr, tb, 0, s, k_mg_cells1, d, b, mode);
 }
 
 int adfb_block_set_mg(int coarseBlk, int fineBlk, const int32_t* mgIFine, const int32_t* mgJFine, const int32_t* mgKFine,
@@ -2046,12 +2003,8 @@ static int adfb_mg_restrict_body(int fineLevel) {
         any = true;
         dim3 tb(32, 4, 1);
         dim3 gr((c.d.nx + 31) / 32, (c.d.ny + 3) / 4, c.d.nz);
-        KT_BEGIN(K_MISC, g.stream);
-        launch_pdl(k_mg_restrict, gr, tb, g.stream, c.d, c.dev, f.d, f.dev, c.mg);
-        KT_END(K_MISC, g.stream);
-        KT_BEGIN(K_MISC, g.stream);
-        launch_pdl(k_mg_corner_rows, dim3(1), dim3(256), g.stream, c.d, c.dev);
-        KT_END(K_MISC, g.stream);
+        launch_kernel(K_MISC, true, gr, tb, 0, g.stream, k_mg_restrict, c.d, c.dev, f.d, f.dev, c.mg);
+        launch_kernel(K_MISC, true, dim3(1), dim3(256), 0, g.stream, k_mg_corner_rows, c.d, c.dev);
         if (launch_bc_levels(c.d, c.dev, c.subfaces, 0, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
     if (!any) return fail("adfb_mg_restrict: no blocks on level %d", cl);
@@ -2071,9 +2024,7 @@ static int adfb_mg_restrict_body(int fineLevel) {
         if (!c.alive || c.level != cl) continue;
         dim3 tb(32, 4, 2);
         dim3 gr((c.d.nx + 31) / 32, (c.d.ny + 3) / 4, (c.d.nz + 1) / 2);
-        KT_BEGIN(K_MISC, g.stream);
-        launch_pdl(k_mg_forcing, gr, tb, g.stream, c.d, c.dev, g.prm.fcoll);
-        KT_END(K_MISC, g.stream);
+        launch_kernel(K_MISC, true, gr, tb, 0, g.stream, k_mg_forcing, c.d, c.dev, g.prm.fcoll);
     }
     CK(cudaGetLastError());
     return 0;
@@ -2099,15 +2050,11 @@ static int adfb_mg_prolong_body(int fineLevel) {
             FaceDev fd = make_face(c.d, sf);
             dim3 tb(32, 4);
             dim3 gr((fd.icEnd - fd.icBeg + 1 + 31) / 32, (fd.jcEnd - fd.jcBeg + 1 + 3) / 4);
-            KT_BEGIN(K_BC, g.stream);
-            launch_pdl(k_mg_corr_halos, gr, tb, g.stream, c.d, c.dev, fd, fact, 5);
-            KT_END(K_BC, g.stream);
+            launch_kernel(K_BC, true, gr, tb, 0, g.stream, k_mg_corr_halos, c.d, c.dev, fd, fact, 5);
         }
         dim3 tb(32, 4, 1);
         dim3 gr((f.d.nx + 31) / 32, (f.d.ny + 3) / 4, f.d.nz);
-        KT_BEGIN(K_MISC, g.stream);
-        launch_pdl(k_mg_prolong, gr, tb, g.stream, f.d, f.dev, c.d, c.dev, c.mg, f.nw);
-        KT_END(K_MISC, g.stream);
+        launch_kernel(K_MISC, true, gr, tb, 0, g.stream, k_mg_prolong, f.d, f.dev, c.d, c.dev, c.mg, f.nw);
         // applyAllBC(secondHalo): second halos on the ground level only
         if (launch_bc_levels(f.d, f.dev, f.subfaces, above_ground(fineLevel) ? 0 : 1, 0, 1, g.stream)) return fail("flow BC launch failed");
     }
@@ -2158,23 +2105,17 @@ static int adfb_mg_prolong_solution_body(int fineLevel) {
             FaceDev fd = make_face(c.d, sf);
             dim3 tb(32, 4);
             dim3 gr((fd.icEnd - fd.icBeg + 1 + 31) / 32, (fd.jcEnd - fd.jcBeg + 1 + 3) / 4);
-            KT_BEGIN(K_BC, g.stream);
-            launch_pdl(k_mg_corr_halos, gr, tb, g.stream, c.d, c.dev, fd, 1.0, f.nw);
-            KT_END(K_BC, g.stream);
+            launch_kernel(K_BC, true, gr, tb, 0, g.stream, k_mg_corr_halos, c.d, c.dev, fd, 1.0, f.nw);
         }
         {
             dim3 tb(32, 4, 1);
             dim3 gr((f.d.nx + 31) / 32, (f.d.ny + 3) / 4, f.d.nz);
-            KT_BEGIN(K_MISC, g.stream);
-            launch_pdl(k_mg_prolong_solution, gr, tb, g.stream, f.d, f.dev, c.d, c.dev, c.mg, f.nw);
-            KT_END(K_MISC, g.stream);
+            launch_kernel(K_MISC, true, gr, tb, 0, g.stream, k_mg_prolong_solution, f.d, f.dev, c.d, c.dev, c.mg, f.nw);
         }
         {
             dim3 tb(32, 4, 2);
             dim3 gr((f.d.NI + 31) / 32, (f.d.NJ + 3) / 4, (f.d.NK + 1) / 2);
-            KT_BEGIN(K_MISC, g.stream);
-            launch_pdl(k_mg_extrapolate, gr, tb, g.stream, f.d, f.dev, f.nw);
-            KT_END(K_MISC, g.stream);
+            launch_kernel(K_MISC, true, gr, tb, 0, g.stream, k_mg_extrapolate, f.d, f.dev, f.nw);
         }
         const bool rans = g.prm.equations == ADFB_RANS;
         if (rans && launch_bc_levels(f.d, f.dev, f.subfaces, 1, 1, 0, g.stream)) return fail("turbulence BC launch failed");
@@ -2267,13 +2208,9 @@ static int kry_apply_op(int op, const double* inDev, double* outDev, long long n
     return 0;
 }
 static int kry_dots(const double* V, long long ld, int nv, const double* w, long long n, double* hOut) {
-    KT_BEGIN(K_MFFD, g.stream);
-    k_multidot<<<ADFB_GMRES_PARTS, 256, 0, g.stream>>>(V, ld, nv, w, n, g.kryRed);
-    KT_END(K_MFFD, g.stream);
+    launch_kernel(K_MFFD, false, ADFB_GMRES_PARTS, 256, 0, g.stream, k_multidot, V, ld, nv, w, n, g.kryRed);
     double* fin = g.kryRed + (size_t)ADFB_GMRES_PARTS * ADFB_GMRES_MAXV;
-    KT_BEGIN(K_MFFD, g.stream);
-    k_multidot_final<<<nv, 256, 0, g.stream>>>(g.kryRed, ADFB_GMRES_PARTS, nv, fin);
-    KT_END(K_MFFD, g.stream);
+    launch_kernel(K_MFFD, false, nv, 256, 0, g.stream, k_multidot_final, g.kryRed, ADFB_GMRES_PARTS, nv, fin);
     return allreduce_fetch(fin, nv, kNcclSum, hOut);
 }
 int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int restart, int maxIts, double rtol, double atol,
@@ -2324,14 +2261,14 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
             if (kry_apply_op(op, xd, w, n)) return 1;
             CK(cudaMemcpyAsync(z, rhs, n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
             GmresCoef c1 = {}; c1.c[0] = 1.0;
-            k_axpy_many<<<nb, 256, 0, g.stream>>>(z, n, 1, c1, -1.0, w, n);   // w = -w + b
+            launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_axpy_many, z, n, 1, c1, -1.0, w, n);   // w = -w + b
             if (kry_dots(w, n, 1, w, n, &bb)) return 1;
             rnorm = sqrt(bb);
             if (!std::isfinite(rnorm)) { rnorm = NAN; break; }
             if (rnorm <= target) break;
         }
         first = false;
-        k_scale_to<<<nb, 256, 0, g.stream>>>(w, 1.0 / rnorm, V, n);
+        launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_scale_to, w, 1.0 / rnorm, V, n);
         std::fill(gg.begin(), gg.end(), 0.0);
         gg[0] = rnorm;
         int j = 0;
@@ -2348,14 +2285,14 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
             if (kry_dots(V, n, j + 1, w, n, hcol.data())) return 1;
             GmresCoef cf = {};
             for (int i = 0; i <= j; i++) cf.c[i] = -hcol[i];
-            k_axpy_many<<<nb, 256, 0, g.stream>>>(V, n, j + 1, cf, 1.0, w, n);
+            launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_axpy_many, V, n, j + 1, cf, 1.0, w, n);
             double ww = 0.0;
             if (kry_dots(w, n, 1, w, n, &ww)) return 1;
             hcol[j + 1] = sqrt(ww);
             bool finite = std::isfinite(hcol[j + 1]);
             for (int i = 0; i <= j; i++) finite = finite && std::isfinite(hcol[i]);
             if (!finite) { its++; rnorm = NAN; stop = true; break; }
-            if (hcol[j + 1] > 0.0) k_scale_to<<<nb, 256, 0, g.stream>>>(w, 1.0 / hcol[j + 1], V + (size_t)(j + 1) * n, n);
+            if (hcol[j + 1] > 0.0) launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_scale_to, w, 1.0 / hcol[j + 1], V + (size_t)(j + 1) * n, n);
             // Givens rotations on the new column
             for (int i = 0; i < j; i++) {
                 const double t = cs[i] * hcol[i] + sn[i] * hcol[i + 1];
@@ -2392,13 +2329,13 @@ int adfb_gmres_solve(int op, const double* rhs, double* x, long long n, int rest
         GmresCoef cy = {};
         for (int i = 0; i < k; i++) cy.c[i] = y[i];
         if (pc) {
-            k_axpy_many<<<nb, 256, 0, g.stream>>>(V, n, k, cy, 0.0, w, n);
+            launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_axpy_many, V, n, k, cy, 0.0, w, n);
             CK(cudaStreamSynchronize(g.stream));
             if (pc(pcCtx, w, z, n)) return fail("adfb_gmres_solve: the preconditioner callback failed");
             GmresCoef c1 = {}; c1.c[0] = 1.0;
-            k_axpy_many<<<nb, 256, 0, g.stream>>>(z, n, 1, c1, 1.0, xd, n);
+            launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_axpy_many, z, n, 1, c1, 1.0, xd, n);
         } else {
-            k_axpy_many<<<nb, 256, 0, g.stream>>>(V, n, k, cy, 1.0, xd, n);
+            launch_kernel(K_MFFD, false, nb, 256, 0, g.stream, k_axpy_many, V, n, k, cy, 1.0, xd, n);
         }
     }
     if (its > 0 && !std::isnan(rnorm)) {   // a non-finite update (the callback's, or an overflowing y) reports NaN as well

@@ -470,44 +470,26 @@ static int launch_dadi(const Dims& d, const BlockDev& b, const AdfbParams& prm, 
     auto thomas = [&](int sd, int nl, int s1, int n1, int s2, int n2) {
         if (sd == 1) {
             const long long items = (long long)((n1 + 31) / 32) * n2 * 5;
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3((unsigned)((items + ADFB_DT_WARPS - 1) / ADFB_DT_WARPS)); cfg.blockDim = dim3(32 * ADFB_DT_WARPS);
-            cfg.dynamicSmemBytes = kDadiTileSmem; cfg.stream = s;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = attr; cfg.numAttrs = 1;
-            cudaLaunchKernelEx(&cfg, k_dadi_thomas_tile, d, b, sd, nl, s1, n1, s2, n2);
+            launch_kernel(K_DADI, true, (unsigned)((items + ADFB_DT_WARPS - 1) / ADFB_DT_WARPS), 32 * ADFB_DT_WARPS, kDadiTileSmem, s,
+                          k_dadi_thomas_tile, d, b, sd, nl, s1, n1, s2, n2);
             return;
         }
-        launch_pdl(k_dadi_thomas, dim3((n1 + 31) / 32, n2, 5), tb, s, d, b, sd, nl, s1, n1, s2, n2);
+        launch_kernel(K_DADI, true, dim3((n1 + 31) / 32, n2, 5), tb, 0, s, k_dadi_thomas, d, b, sd, nl, s1, n1, s2, n2);
     };
     // rows + solve of one direction
     auto solve = [&](int sd, int dirIdx, int nl, int s1, int n1, int s2, int n2) {
-        KT_BEGIN(K_DADI, s);
-        launch_pdl(k_dadi_tri, gc, tc, s, d, b, sd, dirIdx);
-        KT_END(K_DADI, s);
-        KT_BEGIN(K_DADI, s);
+        launch_kernel(K_DADI, true, gc, tc, 0, s, k_dadi_tri, d, b, sd, dirIdx);
         thomas(sd, nl, s1, n1, s2, n2);
-        KT_END(K_DADI, s);
     };
     // j sweep
-    KT_BEGIN(K_DADI, s);
-    launch_pdl(k_dadi_coef<0>, gc, tc, s, d, b, sJ, prm.cfl);
-    KT_END(K_DADI, s);
+    launch_kernel(K_DADI, true, gc, tc, 0, s, k_dadi_coef<0>, d, b, sJ, prm.cfl);
     solve(sJ, 0, d.ny, 1, d.nx, sK, d.nz);
     // i sweep
-    KT_BEGIN(K_DADI, s);
-    launch_pdl(k_dadi_coef<1>, gc, tc, s, d, b, 1, prm.cfl);
-    KT_END(K_DADI, s);
+    launch_kernel(K_DADI, true, gc, tc, 0, s, k_dadi_coef<1>, d, b, 1, prm.cfl);
     solve(1, 1, d.nx, sJ, d.ny, sK, d.nz);
     // k sweep
-    KT_BEGIN(K_DADI, s);
-    launch_pdl(k_dadi_coef<2>, gc, tc, s, d, b, sK, prm.cfl);
-    KT_END(K_DADI, s);
+    launch_kernel(K_DADI, true, gc, tc, 0, s, k_dadi_coef<2>, d, b, sK, prm.cfl);
     solve(sK, 2, d.nz, 1, d.nx, sJ, d.ny);
-    KT_BEGIN(K_DADI, s);
-    launch_pdl(k_dadi_post, gc, tc, s, d, b);
-    KT_END(K_DADI, s);
+    launch_kernel(K_DADI, true, gc, tc, 0, s, k_dadi_post, d, b);
     return (int)cudaGetLastError();
 }

@@ -1011,15 +1011,10 @@ static int launch_flowres_tile(const Dims& d, const BlockDev& b, const AdfbParam
     const int nti = (d.nx + t.TX - 2) / (t.TX - 1), ntj = (d.ny + t.TY - 2) / (t.TY - 1), nkc = (d.nz + t.kChunk - 1) / t.kChunk;
     if (zCount < 0) zCount = nkc - zOff;
     if (zOff < 0 || zCount < 1 || zOff + zCount > nkc) return 1;
-    dim3 grid(nti, ntj, zCount), block(t.nT);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = t.smemBytes; cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    const dim3 grid(nti, ntj, zCount);
     cudaError_t e;
-#define FT_LAUNCH(V, M) e = cudaLaunchKernelEx(&cfg, k_flowres<V, M>, d, b, t, rFil, doDiss, persistFw, nw, mf, maps, zOff)
+#define FT_LAUNCH(V, M) \
+    e = launch_kernel(K_RESID, true, grid, t.nT, t.smemBytes, stream, k_flowres<V, M>, d, b, t, rFil, doDiss, persistFw, nw, mf, maps, zOff)
     if (viscous) { if (merged) FT_LAUNCH(true, true); else FT_LAUNCH(true, false); }
     else { if (merged) FT_LAUNCH(false, true); else FT_LAUNCH(false, false); }
 #undef FT_LAUNCH

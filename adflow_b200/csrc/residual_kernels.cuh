@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(256) k_geom(Dims d, BlockDev b) {
 // disc: the discretisation of the residual that reads ss (residual_discr); scaleRad: directional scaling of the radii
 // (doScaling of timeStep: always on the blockette path, dirScaling .and. currentLevel <= groundLevel on the block path)
 __global__ void __launch_bounds__(256) k_prep(Dims d, BlockDev b, int updateDt, int doRad, int kOff, int kTop, int disc, int scaleRad) {
-    ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_pdl)
+    ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_kernel with pdl)
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int j = blockIdx.y * blockDim.y + threadIdx.y;
     const int k = blockIdx.z * blockDim.z + threadIdx.z + kOff;
@@ -668,9 +668,7 @@ __global__ void __launch_bounds__(256) k_div(Dims d, BlockDev b, double rFil, in
 static int launch_geom(const Dims& d, const BlockDev& b, cudaStream_t stream) {
     dim3 tb(32, 4, 2);
     dim3 g((d.NI + tb.x - 1) / tb.x, (d.NJ + tb.y - 1) / tb.y, (d.NK + tb.z - 1) / tb.z);
-    KT_BEGIN(K_METRICS, stream);
-    k_geom<<<g, tb, 0, stream>>>(d, b);
-    KT_END(K_METRICS, stream);
+    launch_kernel(K_METRICS, false, g, tb, 0, stream, k_geom, d, b);
     return (int)cudaGetLastError();
 }
 
@@ -710,16 +708,11 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     // the same stream ahead of k_prep: the tile kernel's CTAs fill an SM's register file, so the two cannot share SMs and a
     // side stream only added its fork and join.
     if (turbRes) {
-        KT_BEGIN(K_SA, stream);
-        const int rc = launch_sa(d, b, env, mf, 0, INT_MAX, stream);
-        KT_END(K_SA, stream);
-        if (rc) return 1;
+        if (launch_sa(d, b, env, mf, 0, INT_MAX, stream)) return 1;
     }
     if (doRad || (flowRes && doDiss)) {
         dim3 g((d.NI + tb.x - 1) / tb.x, (d.NJ + tb.y - 1) / tb.y, (d.NK + tb.z - 1) / tb.z);
-        KT_BEGIN(K_PREP, stream);
-        launch_pdl(k_prep, g, tb, stream, d, b, updateDt, doRad, 0, INT_MAX, disc, (int)!b.coarse);
-        KT_END(K_PREP, stream);
+        launch_kernel(K_PREP, true, g, tb, 0, stream, k_prep, d, b, updateDt, doRad, 0, INT_MAX, disc, (int)!b.coarse);
     }
     // tile kernel (fused_kernels.cuh): exact central + scalar-JST (+ viscous) flow rows in one launch
     bool fusedDone = false;
@@ -731,9 +724,7 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     // fluxes (rFil /= 0); the central-only stages keep k_faces + k_div, which are cheaper there
     if (flowRes && fused_mode() > 0 && (!persistFw || fusedSmoother == 1 || (fusedSmoother == 2 && doDiss)) && !b.coarse && disc == ADFB_DISS_SCALAR && !dissApprox && !viscApprox && !initWr &&
         !(flags & ADFB_RES_STORE_WALL) && !split_faces()) {
-        KT_BEGIN(K_RESID, stream);
         const int rc = launch_flowres_tile(d, b, prm, env, (int)((b.p - b.w) / d.N), rFil, doDiss, !persistFw, persistFw, stream, mf);
-        KT_END(K_RESID, stream);
         if (rc > 0) return 1;
         fusedDone = rc == 0;
     }
@@ -741,17 +732,14 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
     if (flowRes && doDiss && !fusedDone) {
         dim3 tn(32, 4, 2);
         dim3 g((d.ie + tn.x - 1) / tn.x, (d.je + tn.y - 1) / tn.y, (d.ke + tn.z - 1) / tn.z);
-        KT_BEGIN(K_NODAL, stream);
-        if (gradAos) launch_pdl(k_nodal<true>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
-        else launch_pdl(k_nodal<false>, g, tn, stream, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
-        KT_END(K_NODAL, stream);
+        if (gradAos) launch_kernel(K_NODAL, true, g, tn, 0, stream, k_nodal<true>, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
+        else launch_kernel(K_NODAL, true, g, tn, 0, stream, k_nodal<false>, d, b, (int)(doVisc && !viscApprox), dissApprox, disc);
     }
     if (flowRes && !fusedDone) {
         dim3 tr(32, 4, 1);
         dim3 g((d.il + tr.x - 1) / tr.x, (d.jl + tr.y - 1) / tr.y, (d.kl + tr.z - 1) / tr.z);
         const bool merged = !persistFw;
-        KT_BEGIN(K_RESID, stream);
-#define ADFB_LAUNCH_FACES(V, M, D, A) launch_pdl(k_faces<V, M, D, A>, g, tr, stream, d, b, rFil, doVisc, doDiss)
+#define ADFB_LAUNCH_FACES(V, M, D, A) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<V, M, D, A>, d, b, rFil, doVisc, doDiss)
 #define ADFB_FACES_DISC(V, M, A)                                           \
     do {                                                                   \
         if (disc == ADFB_DISS_SCALAR) ADFB_LAUNCH_FACES(V, M, ADFB_DISS_SCALAR, A); \
@@ -764,34 +752,34 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         if (b.coarse) {   // coarse multigrid level: first-order scalar dissipation, block path only
             if (merged || approx) return 1;
             if (disc == ADFB_UPWIND) {   // inviscidUpwindFlux(fineGrid = .false.): first-order states, fluxes.F90:1532
-                if (viscous) launch_pdl(k_faces<true, false, ADFB_UPWIND, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                else launch_pdl(k_faces<false, false, ADFB_UPWIND, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                if (viscous) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, false, ADFB_UPWIND, 1>, d, b, rFil, doVisc, doDiss);
+                else launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<false, false, ADFB_UPWIND, 1>, d, b, rFil, doVisc, doDiss);
             } else if (disc == ADFB_DISS_SCALAR) {
-                if (viscous) launch_pdl(k_faces<true, false, ADFB_DISS_SCALAR, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                else launch_pdl(k_faces<false, false, ADFB_DISS_SCALAR, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                if (viscous) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, false, ADFB_DISS_SCALAR, 4>, d, b, rFil, doVisc, doDiss);
+                else launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<false, false, ADFB_DISS_SCALAR, 4>, d, b, rFil, doVisc, doDiss);
             } else {
-                if (viscous) launch_pdl(k_faces<true, false, ADFB_DISS_MATRIX, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                else launch_pdl(k_faces<false, false, ADFB_DISS_MATRIX, 4>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                if (viscous) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, false, ADFB_DISS_MATRIX, 4>, d, b, rFil, doVisc, doDiss);
+                else launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<false, false, ADFB_DISS_MATRIX, 4>, d, b, rFil, doVisc, doDiss);
             }
         } else if (storeWall) {  // exact viscous flux + viscSubface%tau/%q planes for the force integration
-            if (disc == ADFB_DISS_SCALAR) launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-            else if (disc == ADFB_DISS_MATRIX) launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-            else launch_pdl(k_faces<true, true, ADFB_UPWIND, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+            if (disc == ADFB_DISS_SCALAR) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_SCALAR, 0, true>, d, b, rFil, doVisc, doDiss);
+            else if (disc == ADFB_DISS_MATRIX) launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_MATRIX, 0, true>, d, b, rFil, doVisc, doDiss);
+            else launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_UPWIND, 0, true>, d, b, rFil, doVisc, doDiss);
         } else if (approx == 0 && viscous && merged && doVisc && split_faces()) {
             // two launches with fewer registers each (ADFB_SPLIT_FACES=1): central + dissipation, then viscous
             if (disc == ADFB_DISS_SCALAR) {
-                launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 2>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 1>, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 2>, d, b, rFil, doVisc, doDiss);
             } else if (disc == ADFB_DISS_MATRIX) {
-                launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                launch_pdl(k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 2>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 1>, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_MATRIX, 0, false, 2>, d, b, rFil, doVisc, doDiss);
             } else {
-                launch_pdl(k_faces<true, true, ADFB_UPWIND, 0, false, 1>, g, tr, stream, d, b, rFil, doVisc, doDiss);
-                launch_pdl(k_faces<true, true, ADFB_UPWIND, 0, false, 2>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_UPWIND, 0, false, 1>, d, b, rFil, doVisc, doDiss);
+                launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_UPWIND, 0, false, 2>, d, b, rFil, doVisc, doDiss);
             }
             splitDone = 1;
         } else if (gradAos) {
-            launch_pdl(k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 0, true>, g, tr, stream, d, b, rFil, doVisc, doDiss);
+            launch_kernel(K_RESID, true, g, tr, 0, stream, k_faces<true, true, ADFB_DISS_SCALAR, 0, false, 0, true>, d, b, rFil, doVisc, doDiss);
         } else if (approx == 0) {
             if (viscous) { if (merged) ADFB_FACES_DISC(true, true, 0); else ADFB_FACES_DISC(true, false, 0); }
             else { if (merged) ADFB_FACES_DISC(false, true, 0); else ADFB_FACES_DISC(false, false, 0); }
@@ -804,12 +792,9 @@ static int launch_residual_core(const Dims& d, const BlockDev& b, const AdfbPara
         }
 #undef ADFB_FACES_DISC
 #undef ADFB_LAUNCH_FACES
-        KT_END(K_RESID, stream);
         dim3 g2((d.nx + tb.x - 1) / tb.x, (d.ny + tb.y - 1) / tb.y, (d.nz + tb.z - 1) / tb.z);
-        KT_BEGIN(K_DIV, stream);
-        if (merged) launch_pdl(k_div<true>, g2, tb, stream, d, b, rFil, persistFw, splitDone ? 2 : 0);
-        else launch_pdl(k_div<false>, g2, tb, stream, d, b, rFil, persistFw, initWr);
-        KT_END(K_DIV, stream);
+        if (merged) launch_kernel(K_DIV, true, g2, tb, 0, stream, k_div<true>, d, b, rFil, persistFw, splitDone ? 2 : 0);
+        else launch_kernel(K_DIV, true, g2, tb, 0, stream, k_div<false>, d, b, rFil, persistFw, initWr);
     }
     return (int)cudaGetLastError();
 }

@@ -358,30 +358,22 @@ static int launch_sa_block(const Dims& d, const BlockDev& b, const AdfbParams& p
         const BcList L = make_bc_list(d, subs, q0);
         int ma = 1, mb = 1;
         for (int q = 0; q < L.n; q++) { ma = std::max(ma, L.f[q].icEnd - L.f[q].icBeg + 1); mb = std::max(mb, L.f[q].jcEnd - L.f[q].jcBeg + 1); }
-        KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_bmt, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)L.n), dim3(32, 4), s, d, b, L);
-        KT_END(K_SASOLVE, s);
+        launch_kernel(K_SASOLVE, true, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)L.n), dim3(32, 4), 0, s, k_sa_bmt, d, b, L);
     }
     const double factor = 1.0 + (1.0 - prm.alfaTurb) / prm.alfaTurb;
     {
         dim3 tr(32, 4, 1);
         dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, d.nz);
-        KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_rhs, g, tr, s, d, b, factor);
-        KT_END(K_SASOLVE, s);
+        launch_kernel(K_SASOLVE, true, g, tr, 0, s, k_sa_rhs, d, b, factor);
     }
     const dim3 tl(32, 1), tc(32, 4, 1), gc((d.nx + 31) / 32, (d.ny + 3) / 4, d.nz);
     auto sweep = [&](int axis, int sd, int nl, int s1, int n1, int s2, int n2, int mult) {
-        KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_coef, gc, tc, s, d, b, axis, sd);
-        KT_END(K_SASOLVE, s);
-        KT_BEGIN(K_SASOLVE, s);
+        launch_kernel(K_SASOLVE, true, gc, tc, 0, s, k_sa_coef, d, b, axis, sd);
         const int part = adfb_part_lanes(nl);
-        if (part == 8 && nl <= 96) launch_pdl(k_sa_thomas_part<8, 12>, (n1 * n2 + 3) / 4, 32, s, d, b, sd, nl, s1, n1, s2, n2, mult);
-        else if (part == 8) launch_pdl(k_sa_thomas_part<8, 16>, (n1 * n2 + 3) / 4, 32, s, d, b, sd, nl, s1, n1, s2, n2, mult);
-        else if (part == 16) launch_pdl(k_sa_thomas_part<16, 16>, (n1 * n2 + 1) / 2, 32, s, d, b, sd, nl, s1, n1, s2, n2, mult);
-        else launch_pdl(k_sa_thomas, dim3((n1 + 31) / 32, n2), tl, s, d, b, sd, nl, s1, n1, s2, n2, mult);
-        KT_END(K_SASOLVE, s);
+        if (part == 8 && nl <= 96) launch_kernel(K_SASOLVE, true, (n1 * n2 + 3) / 4, 32, 0, s, k_sa_thomas_part<8, 12>, d, b, sd, nl, s1, n1, s2, n2, mult);
+        else if (part == 8) launch_kernel(K_SASOLVE, true, (n1 * n2 + 3) / 4, 32, 0, s, k_sa_thomas_part<8, 16>, d, b, sd, nl, s1, n1, s2, n2, mult);
+        else if (part == 16) launch_kernel(K_SASOLVE, true, (n1 * n2 + 1) / 2, 32, 0, s, k_sa_thomas_part<16, 16>, d, b, sd, nl, s1, n1, s2, n2, mult);
+        else launch_kernel(K_SASOLVE, true, dim3((n1 + 31) / 32, n2), tl, 0, s, k_sa_thomas, d, b, sd, nl, s1, n1, s2, n2, mult);
     };
     sweep(1, sJ, d.ny, 1, d.nx, sK, d.nz, 1);   // j lines
     sweep(0, 1, d.nx, sJ, d.ny, sK, d.nz, 1);   // i lines
@@ -389,9 +381,7 @@ static int launch_sa_block(const Dims& d, const BlockDev& b, const AdfbParams& p
     {
         dim3 tb(32, 4, 2);
         dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, (d.nz + 1) / 2);
-        KT_BEGIN(K_SASOLVE, s);
-        launch_pdl(k_sa_update, g, tb, s, d, b);
-        KT_END(K_SASOLVE, s);
+        launch_kernel(K_SASOLVE, true, g, tb, 0, s, k_sa_update, d, b);
     }
     if (launch_bc_levels(d, b, subs, 1, 1, 0, s)) return 1;
     return (int)cudaGetLastError();

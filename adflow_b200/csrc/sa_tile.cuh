@@ -463,7 +463,6 @@ static int launch_sa(const Dims& d, const BlockDev& b, const LaunchEnv& env, Mff
     if (nPlanes <= 0) return 0;
     const SaTile t = sa_tile_choose(d, nPlanes, env.nSM > 0 ? env.nSM : 1, env.saCtasPerSM > 0 ? env.saCtasPerSM : 1);
     const dim3 g((d.nx + t.TX - 1) / t.TX, (d.ny + t.TY - 1) / t.TY, (nPlanes + t.kChunk - 1) / t.kChunk);
-    k_sa<<<g, t.nT, SA_SMEM_BYTES, stream>>>(d, b, t, mf, kOff, kTop);
-    return (int)cudaGetLastError();
+    return (int)launch_kernel(K_SA, false, g, t.nT, SA_SMEM_BYTES, stream, k_sa, d, b, t, mf, kOff, kTop);
 }
 #endif

@@ -744,9 +744,7 @@ static int launch_bc_levels(const Dims& d, const BlockDev& b, const std::vector<
         int ma = 1, mb = 1;
         auto flush = [&]() {
             if (!lv.n) return;
-            KT_BEGIN(K_BC, s);
-            launch_pdl(k_bc_level, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)lv.n), dim3(32, 4), s, d, b, lv, secondHalo);
-            KT_END(K_BC, s);
+            launch_kernel(K_BC, true, dim3((ma + 31) / 32, (mb + 3) / 4, (unsigned)lv.n), dim3(32, 4), 0, s, k_bc_level, d, b, lv, secondHalo);
             lv.n = 0; ma = 1; mb = 1;
         };
         for (size_t q = 0; q < items.size(); q++) {
@@ -787,31 +785,19 @@ static int launch_residual_averaging(const Dims& d, const BlockDev& b, const Adf
     {
         dim3 tb(32, 4, 2);
         dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, (d.nz + 1) / 2);
-        KT_BEGIN(K_RK, s);
-        launch_pdl(k_resavg_rfl, g, tb, s, d, b);
-        KT_END(K_RK, s);
-        KT_BEGIN(K_RK, s);
-        launch_pdl(k_resavg_eps, g, tb, s, d, b, rfl0);
-        KT_END(K_RK, s);
+        launch_kernel(K_RK, true, g, tb, 0, s, k_resavg_rfl, d, b);
+        launch_kernel(K_RK, true, g, tb, 0, s, k_resavg_eps, d, b, rfl0);
     }
     dim3 tb(32, 2);
     auto run = [&](int dir, long long sd, int n, long long s1, int n1, long long s2, int n2) {
         if (n <= 1) return;
-        KT_BEGIN(K_RK, s);
         int LP = 0; size_t smem = 0;
         const int lpc = lines_per_cta((long long)n1 * n2, n, 8, ADFB_RA_THREADS / 5, kResavgSmemMax, env.nSM, &LP, &smem);
-        if (lpc) {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3((unsigned)(((long long)n1 * n2 + lpc - 1) / lpc)); cfg.blockDim = dim3(ADFB_RA_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attr[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = attr; cfg.numAttrs = 1;
-            cudaLaunchKernelEx(&cfg, k_resavg_lines, d, b, dir, sd, n, s1, n1, s2, n2, lpc, LP);
-        } else {   // not even one line fits into shared memory (n >= 3520 cells)
-            launch_pdl(k_resavg_sweep, dim3((n1 + 31) / 32, (n2 + 1) / 2, 5), tb, s, d, b, dir, sd, n, s1, n1, s2, n2);
-        }
-        KT_END(K_RK, s);
+        if (lpc)
+            launch_kernel(K_RK, true, (unsigned)(((long long)n1 * n2 + lpc - 1) / lpc), ADFB_RA_THREADS, smem, s, k_resavg_lines, d, b, dir, sd, n,
+                          s1, n1, s2, n2, lpc, LP);
+        else   // not even one line fits into shared memory (n >= 3520 cells)
+            launch_kernel(K_RK, true, dim3((n1 + 31) / 32, (n2 + 1) / 2, 5), tb, 0, s, k_resavg_sweep, d, b, dir, sd, n, s1, n1, s2, n2);
     };
     run(0, 1, d.nx, d.sJ, d.ny, d.sK, d.nz);
     run(1, d.sJ, d.ny, 1, d.nx, d.sK, d.nz);
@@ -827,17 +813,11 @@ static int launch_rk_update(const Dims& d, const BlockDev& b, const AdfbParams& 
     dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, (d.nz + 1) / 2);
     const int nw = nwOverride ? nwOverride : (prm.equations == ADFB_RANS ? 6 : 5);   // 5: eddy viscosity frozen (coarse levels)
     if (smooth) {
-        KT_BEGIN(K_RK, s);
-        launch_pdl(k_rk_scale, g, tb, s, d, b, tmp);
-        KT_END(K_RK, s);
+        launch_kernel(K_RK, true, g, tb, 0, s, k_rk_scale, d, b, tmp);
         if (launch_residual_averaging(d, b, prm, env, s)) return 1;
-        KT_BEGIN(K_RK, s);
-        launch_pdl(k_rk_update, g, tb, s, d, b, 0, tmp, nw, 0);
-        KT_END(K_RK, s);
+        launch_kernel(K_RK, true, g, tb, 0, s, k_rk_update, d, b, 0, tmp, nw, 0);
     } else {
-        KT_BEGIN(K_RK, s);
-        launch_pdl(k_rk_update, g, tb, s, d, b, 1, tmp, nw, 0);
-        KT_END(K_RK, s);
+        launch_kernel(K_RK, true, g, tb, 0, s, k_rk_update, d, b, 1, tmp, nw, 0);
     }
     return (int)cudaGetLastError();
 }
@@ -848,9 +828,7 @@ static int launch_dadi_update(const Dims& d, const BlockDev& b, const AdfbParams
         if (launch_residual_averaging(d, b, prm, env, s)) return 1;
     dim3 tb(32, 4, 2);
     dim3 g((d.nx + 31) / 32, (d.ny + 3) / 4, (d.nz + 1) / 2);
-    KT_BEGIN(K_RK, s);
-    launch_pdl(k_rk_update, g, tb, s, d, b, 0, 0.0, nwOverride ? nwOverride : (prm.equations == ADFB_RANS ? 6 : 5), 1);
-    KT_END(K_RK, s);
+    launch_kernel(K_RK, true, g, tb, 0, s, k_rk_update, d, b, 0, 0.0, nwOverride ? nwOverride : (prm.equations == ADFB_RANS ? 6 : 5), 1);
     return (int)cudaGetLastError();
 }
 
@@ -863,9 +841,7 @@ static int launch_wall_forces(const Dims& d, const BlockDev& b, const std::vecto
         FaceDev f = make_face(d, sf);
         const int dir = (sf.faceId - 1) / 2, isMin = (sf.faceId % 2) == 1;
         const int la = dir == 0 ? d.jl : d.il, lb = dir == 2 ? d.jl : d.kl;
-        KT_BEGIN(K_MISC, s);
-        launch_pdl(k_wall_forces, 1, 256, s, d, b, f, sf.iblank, dir, isMin, la, lb, viscWall ? 1 : 0, rp[0], rp[1], rp[2], pRef, acc);
-        KT_END(K_MISC, s);
+        launch_kernel(K_MISC, true, 1, 256, 0, s, k_wall_forces, d, b, f, sf.iblank, dir, isMin, la, lb, viscWall ? 1 : 0, rp[0], rp[1], rp[2], pRef, acc);
     }
     return (int)cudaGetLastError();
 }

@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(256) k_metrics(Dims d, BlockDev b, double fact
 // p on [pLo,pHi] (owned, or 0:ib with halos), rlv/rev on [vLo,vHi] (owned, or 1:ie with halos)
 // kOff / kTop: the planes lo + kOff .. kTop only (slab pipeline of adfb_form_function); 0 / INT_MAX: all of them
 __global__ void __launch_bounds__(256) k_state_prep(Dims d, BlockDev b, int includeHalos, int nw, int etot, int kOff, int kTop) {
-    ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_pdl)
+    ADFB_PDL_SYNC();  // launched with programmatic stream serialization (launch_kernel with pdl)
     const int lo = includeHalos ? 0 : 2;
     const int i = blockIdx.x * blockDim.x + threadIdx.x + lo;
     const int j = blockIdx.y * blockDim.y + threadIdx.y + lo;
@@ -380,18 +380,14 @@ static int launch_vec(const Dims& d, const BlockDev& b, int nw, double* vec, int
     const long long nOwned = (long long)d.nx * d.ny * d.nz;
     // mode 3 covers the whole box per variable, 4 and 5 the owned cells, 6 the box cells
     const long long n = mode == 3 ? d.N * nw : mode == 6 ? d.N : mode >= 4 ? nOwned : nOwned * nw;
-    KT_BEGIN(K_VEC, stream);
-    k_vec<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d, b, nw, vec, mode, cf);
-    KT_END(K_VEC, stream);
+    launch_kernel(K_VEC, false, (unsigned)((n + 255) / 256), 256, 0, stream, k_vec, d, b, nw, vec, mode, cf);
     return (int)cudaGetLastError();
 }
 
 static int launch_metrics(const Dims& d, const BlockDev& b, int rightHanded, cudaStream_t stream) {
     dim3 tb(32, 4, 2);
     dim3 g((d.ie + 1 + tb.x - 1) / tb.x, (d.je + 1 + tb.y - 1) / tb.y, (d.ke + 1 + tb.z - 1) / tb.z);
-    KT_BEGIN(K_METRICS, stream);
-    k_metrics<<<g, tb, 0, stream>>>(d, b, rightHanded ? 0.5 : -0.5);
-    KT_END(K_METRICS, stream);
+    launch_kernel(K_METRICS, false, g, tb, 0, stream, k_metrics, d, b, rightHanded ? 0.5 : -0.5);
     return (int)cudaGetLastError();
 }
 
@@ -400,24 +396,18 @@ static int launch_state_prep(const Dims& d, const BlockDev& b, const AdfbParams&
     dim3 tb(32, 4, 2);
     const int ni = includeHalos ? d.NI : d.nx, nj = includeHalos ? d.NJ : d.ny, nk = includeHalos ? d.NK : d.nz;
     dim3 g((ni + tb.x - 1) / tb.x, (nj + tb.y - 1) / tb.y, (nk + tb.z - 1) / tb.z);
-    KT_BEGIN(K_STATE, stream);
-    launch_pdl(k_state_prep, g, tb, stream, d, b, includeHalos ? 1 : 0, prm.equations == ADFB_RANS ? 6 : 5, etot ? 1 : 0, 0, INT_MAX);
-    KT_END(K_STATE, stream);
+    launch_kernel(K_STATE, true, g, tb, 0, stream, k_state_prep, d, b, includeHalos ? 1 : 0, prm.equations == ADFB_RANS ? 6 : 5, etot ? 1 : 0, 0, INT_MAX);
     return (int)cudaGetLastError();
 }
 
 // pass 1 of the monitor reduction on one block, into its own nPart x ADFB_MON_N slot of the partials
 static int launch_norms_partial(const Dims& d, const BlockDev& b, const MonCoef& mc, unsigned what, double* part, int nPart,
                                 cudaStream_t stream) {
-    KT_BEGIN(K_NORMS, stream);
-    k_norms_partial<<<nPart, 256, 0, stream>>>(d, b, mc, what, part, nPart);
-    KT_END(K_NORMS, stream);
+    launch_kernel(K_NORMS, false, nPart, 256, 0, stream, k_norms_partial, d, b, mc, what, part, nPart);
     return (int)cudaGetLastError();
 }
 static int launch_norms_final(const double* part, int nPart, long long stride, int nBlk, unsigned what, double hInf, double* out,
                               cudaStream_t stream) {
-    KT_BEGIN(K_NORMS, stream);
-    k_norms_final<<<1, 256, 0, stream>>>(part, nPart, stride, nBlk, what, hInf, out);
-    KT_END(K_NORMS, stream);
+    launch_kernel(K_NORMS, false, 1, 256, 0, stream, k_norms_final, part, nPart, stride, nBlk, what, hInf, out);
     return (int)cudaGetLastError();
 }

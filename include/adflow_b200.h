@@ -275,6 +275,9 @@ int adfb_set_uniform_flow(int level, double muInf, double eddyVisInfRatio);
 /* blocks until the library stream is idle (the reference is synchronous: needed only before timing or host reads
    that bypass the download calls) */
 int adfb_synchronize(void);
+/* Diagnostics the library exports beside this interface: adfb_launch_count() returns the number of kernels the library
+   has launched, one per kernel -- a launch recorded while a CUDA graph is captured counted, and a graph's kernels
+   counted again each time it is replayed. */
 /* wallIntegrationFace / getForces (src/solver/surfaceIntegrations.F90:406-881, src/warping/getForces.F90):
    out = Fp(3), Fv(3), Mp(3), Mv(3) summed over the wall subfaces (viscous walls: pressure + viscous, Euler walls:
    pressure) of all blocks of `level` on all ranks; moments about refPoint; forces scaled by pRef like the
